@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """bench.py -- FK + end-effector Jacobian throughput of the Kuka iiwa 7-DoF (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 One *step* = one pass of the hot path (one `drmb200_fk_jacobian` launch: pos, quat, J_lin, J_ang
 of `iiwa_link_ee`) over one batch of 65 536 synthetic joint configurations (BASELINE.json
 configs[1]).  Inputs are resident in HBM before the timed region; the step cycles through ROTATE
-distinct buffer sets (> the 126 MB L2) so no launch finds its data in L2.
+distinct buffer sets (> the 50 MB L2 of an H100) so no launch finds its data in L2.
 
 Launch pattern of the headline number: the K launches are replayed from a CUDA graph (the per-launch
 Python/ctypes overhead would otherwise exceed the ~3 us kernel) as four independent chains (graph
@@ -27,16 +27,21 @@ Extra keys on the JSON line (see DESIGN.md "Measurement"):
   roofline_large_batch  the same kernel on 2^22 configurations per launch (the asymptotic figure)
   launch_modes        us per launch: one stream + PDL, one stream, 4 graph branches, 4 branches + PDL (the headline)
   e2e                 same metric through the host-buffer C-ABI call (H2D + kernel + D2H per step)
-  cpu_baseline        the UNMODIFIED reference (baseline/_ref) on the host cores, bounded sample
+  cpu_baseline        the UNMODIFIED reference (oracle/_ref/reference) on the host cores, bounded sample
   cpu_baseline_port   the vectorised torch CPU port of the same algorithm (oracle/drm_oracle.py)
   clocks              nvidia-smi SM clocks / throttle reasons sampled during the timed regions
 
 `--impl reference` times the reference's own CPU implementation through its public API
-(`DifferentiableRobotModel.compute_endeffector_jacobian`, unmodified, installed into baseline/_ref by
-`__graft_entry__.build()`; its third-party XML-parser dependency is replaced by oracle/refshim) --
-rank 0 only.
+(`DifferentiableRobotModel.compute_endeffector_jacobian`, unmodified, installed into oracle/_ref/reference by
+`__graft_entry__.build()` where the reference sources are available; its third-party XML-parser dependency is replaced
+by oracle/refshim) -- rank 0 only.
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed path computed in its last step -- the arrays a
+caller of `compute_fk_and_jacobian` receives for that step's 65 536 configurations -- as DIR/{pos,quat,jac_lin,jac_ang}.npy (float32, 12.8 MB in all).  Inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
+import atexit
 import json
 import os
 import statistics
@@ -54,12 +59,12 @@ BATCH = 65536                 # BASELINE.json configs[1]
 EE_LINK = "iiwa_link_ee"
 N_DOF = 7
 BYTES_PER_CONFIG = 28 * N_DOF + 28      # 4n (q) + 12 (pos) + 16 (quat) + 24n (J_lin, J_ang) = 224
-ROTATE = 16                   # 16 x 14.7 MB = 235 MB of distinct buffers > 126 MB L2
+ROTATE = 16                   # 16 x 14.7 MB = 235 MB of distinct buffers > 50 MB L2 (H100)
 GRAPH_NODES = 512
 REPS = 11
 METRIC = "FK+Jacobian configs/sec (Kuka iiwa 7-DoF)"
 UNIT = "configs/s"
-REF_DIR = os.path.join(REPO, "baseline", "_ref")
+REF_DIR = os.path.join(REPO, "oracle", "_ref", "reference")
 REF_SHIM = os.path.join(REPO, "oracle", "refshim")     # stand-in for the reference's urdf_parser_py dependency
 
 
@@ -72,7 +77,7 @@ def bench_config(n_gpus):
             "parallelism": f"batch-sharded x{n_gpus}, no data-path collective",
             "inputs": "q ~ U(joint limits), seeded per rank",
             "l2_policy": f"GPU arm: inputs / outputs rotate over {ROTATE} distinct buffer sets "
-                         f"({ROTATE * BATCH * BYTES_PER_CONFIG / 1e6:.0f} MB) > the 126 MB L2, no launch finds its data in L2"}
+                         f"({ROTATE * BATCH * BYTES_PER_CONFIG / 1e6:.0f} MB) > the 50 MB L2, no launch finds its data in L2"}
 
 
 def measured_peak_gbs():
@@ -81,7 +86,7 @@ def measured_peak_gbs():
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not a measured peak"
 
 
 def sample_q(limits, batch, seed):
@@ -93,7 +98,8 @@ def sample_q(limits, batch, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons every 100 ms while the timed regions run."""
+    """nvidia-smi clocks / throttle reasons every 100 ms while the timed regions run (read-only queries; the sampler
+    process is stopped at exit even when the benchmark fails)."""
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
@@ -104,10 +110,19 @@ class ClockSampler:
             self.proc = subprocess.Popen(
                 ["nvidia-smi", f"--id={gpu_index}", f"--query-gpu={self.FIELDS}", "--format=csv,noheader,nounits",
                  "-lms", "100"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.stop)
             self.thread = threading.Thread(target=self._read, daemon=True)
             self.thread.start()
         except Exception:
             self.proc = None
+
+    def stop(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.terminate()
+            try:
+                self.proc.wait(timeout=5)
+            except subprocess.TimeoutExpired:
+                self.proc.kill()
 
     def _read(self):
         for line in self.proc.stdout:
@@ -122,7 +137,7 @@ class ClockSampler:
     def summary(self):
         if self.proc is not None:
             time.sleep(0.15)
-            self.proc.terminate()
+            self.stop()
         parsed = []
         for ts, line in self.rows:
             parts = [p.strip() for p in line.split(",")]
@@ -144,13 +159,13 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------
-# CPU arms: the unmodified reference (baseline/_ref) and the vectorised port (oracle/)
+# CPU arms: the unmodified reference (oracle/_ref/reference) and the vectorised port (oracle/)
 # ------------------------------------------------------------------------------------------------
 _REF_MODEL = None
 
 
 def reference_model():
-    """The reference's own DifferentiableKUKAiiwa on the CPU, imported from baseline/_ref (None if not installed)."""
+    """The reference's own DifferentiableKUKAiiwa on the CPU, imported from oracle/_ref/reference (None if not installed)."""
     global _REF_MODEL
     if _REF_MODEL is None:
         if not os.path.isdir(os.path.join(REF_DIR, "differentiable_robot_model")):
@@ -200,7 +215,7 @@ def pick_threads(call, q):
 
 
 def cpu_arm(kind):
-    """(call, limits, description) of a CPU implementation: 'reference' = baseline/_ref, 'port' = oracle/drm_oracle.py."""
+    """(call, limits, description) of a CPU implementation: 'reference' = oracle/_ref/reference, 'port' = oracle/drm_oracle.py."""
     import differentiable_robot_model_b200 as drm
     ours = drm.DifferentiableKUKAiiwa(device="cpu")          # host-side model only: joint limits + URDF path
     limits = ours.get_joint_limits()
@@ -209,7 +224,7 @@ def cpu_arm(kind):
         if model is None:
             return None, limits, None
         return (lambda q: _reference_call(model, q)), limits, \
-            "the UNMODIFIED reference (baseline/_ref, DifferentiableKUKAiiwa.compute_endeffector_jacobian, torch CPU fp32, " \
+            "the UNMODIFIED reference (oracle/_ref/reference, DifferentiableKUKAiiwa.compute_endeffector_jacobian, torch CPU fp32, " \
             "per-element Python quaternion loop as shipped)"
     from oracle import drm_oracle as O
     robot = O.load_robot(ours.urdf_path, torch.float32)
@@ -246,7 +261,7 @@ def run_reference_arm(args):
         args.steps = 20
     kind = "reference"
     call, limits, what = cpu_arm("reference")
-    if call is None:                                         # baseline/_ref missing: the port is the stand-in, and says so
+    if call is None:                                         # reference not installed: the port is the stand-in, and says so
         kind = "port"
         call, limits, what = cpu_arm("port")
     cores = pick_threads(call, sample_q(limits, 512, 3))
@@ -284,6 +299,8 @@ def main():
     ap.add_argument("--no-large", action="store_true")
     ap.add_argument("--no-modes", action="store_true")
     ap.add_argument("--no-sharded", action="store_true", help="skip the sharded BASELINE configs 4 and 5 (scripts/bench_sharded.py)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -334,6 +351,15 @@ def main():
 
     def step(i):
         engine.fk_jacobian_raw(topo, ee, table, qs[i % ROTATE], out=outs[i % ROTATE])
+
+    def dump_last_step(path, i):
+        """Step i read qs[i % ROTATE] and wrote outs[i % ROTATE]; every step on that buffer set computes the same values."""
+        import numpy as np
+        os.makedirs(path, exist_ok=True)
+        torch.cuda.synchronize(dev)
+        names = ("pos", "quat", "jac_lin", "jac_ang")
+        for name, t in zip(names, outs[i % ROTATE]):
+            np.save(os.path.join(path, name + ".npy"), t.detach().cpu().numpy().astype(np.float32))
 
     stream = torch.cuda.Stream(device=dev)
     sampler = ClockSampler(local_rank) if rank == 0 else None
@@ -427,6 +453,8 @@ def main():
         if sampler:
             sampler.mark_end()
         elapsed_ms = job_ms(region_ms)
+        if args.dump_outputs and rank == 0:
+            dump_last_step(args.dump_outputs, args.steps - 1)
 
         modes = None
         if not args.no_modes:
@@ -466,14 +494,6 @@ def main():
     }
     if modes is not None:
         result["launch_modes"] = modes
-
-    if rank == 0:
-        prof = os.path.join(REPO, "profiles", "fk_jacobian_traffic.json")
-        if os.path.exists(prof):
-            try:
-                result["roofline"]["traffic"] = json.load(open(prof)).get("dram_bytes_per_launch_batch65536")
-            except Exception:
-                pass
 
     # ---- asymptotic figure: 2^22 configurations per launch -----------------------------------------
     if not args.no_large and rank == 0:

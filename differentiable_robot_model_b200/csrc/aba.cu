@@ -1,4 +1,4 @@
-// aba.cu -- batched articulated-body forward dynamics (sm_100a).
+// aba.cu -- batched articulated-body forward dynamics (sm_90a).
 //
 // Replaces, in ONE launch, DifferentiableRobotModel.compute_forward_dynamics (robot_model.py:488-624):
 // update_kinematic_state (robot_model.py:140-195), the bias pass (:537-545), the articulated-inertia pass
@@ -109,13 +109,9 @@ __device__ __forceinline__ void sub_outer(M3& m, V3 x, V3 y) {      // m -= x y^
 }
 __device__ __forceinline__ M3 conj_by(const M3& M, const M3& Y) { return mulNT(mul(M, Y), M); }   // M Y M^T
 
-// ---- element-wise PAIR of two 3x3 blocks (lo | hi) in packed FP32x2 registers -------------------------------------
+// ---- element-wise PAIR of two 3x3 blocks (lo | hi) as f32x2 lanes --------------------------------------------------
 struct M3PP { f32x2 a00, a01, a02, a10, a11, a12, a20, a21, a22; };
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return pk2(__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)); }
 __device__ __forceinline__ float hsum2(f32x2 v) { float lo, hi; upk2(v, lo, hi); return lo + hi; }
 __device__ __forceinline__ M3PP pkm(const M3& lo, const M3& hi) {
     M3PP r;
@@ -276,9 +272,9 @@ aba_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ Fol
         }
 
         // ---- pass 2: leaves -> root, articulated inertias (robot_model.py:547-596) ---------------------------
-        // Packed FP32x2: the 6x6 travels as two element-wise PAIRS of 3x3 blocks, AB = (A | B) and CD = (C | D) -- both
+        // f32x2 pairs: the 6x6 travels as two element-wise PAIRS of 3x3 blocks, AB = (A | B) and CD = (C | D) -- both
         // blocks of a pair see the same rotation M . M^T, the same left cross product with r and the same left factor of
-        // the rank-1 update, so those cost one FFMA2 per two scalar FMAs.
+        // the rank-1 update, so each of those operations is written once for both blocks.
         {
             M3PP cAB = zero_pp(), cCD = zero_pp();       // contribution of link i+1 to its parent i, through registers
             V3 c_pang = zero, c_plin = zero;

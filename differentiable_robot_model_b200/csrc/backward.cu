@@ -1,4 +1,4 @@
-// backward.cu -- analytic reverse-mode kernels for FK/Jacobian and RNEA (sm_100a).
+// backward.cu -- analytic reverse-mode kernels for FK/Jacobian and RNEA (sm_90a).
 //
 // The reference differentiates its per-link op graph with torch autograd (about 7 k graph nodes for one
 // Kuka RNEA).  Here each backward is ONE launch that re-walks the chain / tree per configuration and
@@ -192,7 +192,7 @@ fk_jacobian_backward_kernel(const __grid_constant__ PathProgram prog, const FkBw
 __global__ void reduce_partials_kernel(const float* __restrict__ partials, int n_blocks, int n_entries,
                                        float* __restrict__ table_grad) {
     // one warp per table entry: lanes stride over the CTA partials (fixed assignment -> fixed summation order),
-    // then a shuffle tree.  (One thread per entry looping over ~1200 partials took 35 us, longer than the
+    // then a shuffle tree.  (One thread per entry looping over ~1000 partials took longer than the
     // single-sweep backward kernel it follows.)
     // launched as a programmatic dependent of the adjoint kernel before it on the stream (launch_reduce): its set-up
     // overlaps that kernel's tail, and this wait returns when that grid has completed and its partials are visible

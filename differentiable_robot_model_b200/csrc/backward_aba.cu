@@ -1,4 +1,4 @@
-// backward_aba.cu -- analytic adjoint of the articulated-body forward-dynamics kernel (sm_100a).
+// backward_aba.cu -- analytic adjoint of the articulated-body forward-dynamics kernel (sm_90a).
 //
 // The reference differentiates its per-link op graph of compute_forward_dynamics (robot_model.py:488-624) with
 // autograd; this kernel evaluates the hand-derived reverse-mode recursions instead (stated and verified against
@@ -15,7 +15,8 @@
 // Per link and configuration 33 floats stay in shared memory (slot-major): cos sin | w v | pA -> pA-bar | u |
 // al a -> U-bar | adjoint accumulator (6) | d-bar u-bar | c-bar (4).  The 6x6 articulated inertia IA_i (36 floats, later
 // overwritten by its adjoint) lives in a per-CTA slice of a GLOBAL scratch instead: the CTAs are persistent, so the whole
-// scratch is (#CTAs x links x 36 x 32 floats, 27 MB for the Kuka) and stays resident in the 126 MB L2; every access is a
+// scratch is (#CTAs x links x 36 x 32 floats, about 21 MB for the Kuka at five CTAs on each of 132 SMs) and stays
+// resident in the 50 MB L2; every access is a
 // coalesced 128-byte line of lane-private values.  With IA in shared memory (69 floats per link) only two single-warp CTAs
 // fit per SM -- two of the four schedulers idle; this layout runs four to five.
 // Table gradients: per-CTA accumulators in canonical frames, un-permuted into per-CTA partial tables, then the

@@ -4,7 +4,7 @@
 
 namespace drm {
 
-constexpr int BWD_MAX_GRID = 148 * 8;         // upper bound of persistent CTAs (workspace sizing)
+constexpr int BWD_MAX_GRID = 132 * 8;         // upper bound of persistent CTAs (workspace sizing; H100: 132 SMs)
 constexpr size_t BWD_SMEM_BUDGET = 200 * 1024;
 constexpr float GRAVITY_B = 9.81f;
 

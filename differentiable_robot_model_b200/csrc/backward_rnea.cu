@@ -1,4 +1,4 @@
-// backward_rnea.cu -- analytic reverse-mode kernels for RNEA inverse dynamics (sm_100a).
+// backward_rnea.cu -- analytic reverse-mode kernels for RNEA inverse dynamics (sm_90a).
 //
 // See backward.cu for the common design (recompute instead of save, deterministic table-gradient reduction,
 // canonical joint frames) and oracle/adjoint_proto.py for the recursions in executable form.
@@ -473,7 +473,7 @@ rnea_backward_inertial_kernel(const __grid_constant__ TreeProgram prog, const Rn
 }
 
 // =============================================================================================
-// RNEA backward on a serial chain: two sweeps, packed FP32x2, TMA-staged tiles
+// RNEA backward on a serial chain: two sweeps, f32x2 pair, TMA-staged tiles
 // =============================================================================================
 // For robots whose links form one chain (parent of link i is link i - 1: Kuka iiwa, Franka Panda, ...) the four passes of
 // rnea_backward_kernel collapse into TWO sweeps (oracle/adjoint_proto.py: inverse_dynamics_backward_chain states them
@@ -487,7 +487,7 @@ rnea_backward_inertial_kernel(const __grid_constant__ TreeProgram prog, const Rn
 //     per link instead of 13 + 25.
 // M = F Rz(theta) is never formed: x -> Rz^T (F^T x), x -> F (Rz x).  For y = M^T x with adjoint y-bar the joint-angle
 // gradient is (y-bar x y).z and the F gradient x (Rz y-bar)^T, so no 3x3 M-bar is accumulated for theta either.
-// Velocity- and acceleration-level vectors (and their adjoints) go through the same maps as FP32x2 PAIRS (FFMA2).
+// Velocity- and acceleration-level vectors (and their adjoints) go through the same maps as f32x2 PAIRS.
 // The q / qd / qdd / g_tau row tiles arrive by TMA bulk copies on an mbarrier and the three input-gradient tiles leave by
 // bulk stores FROM THE SAME shared memory: each thread has read q_k, qd_k, qdd_k of its row before it writes the gradient
 // there, so the tiles alias (4 instead of 7 row tiles).  Rows past the end of the batch are zero-filled: with g = 0 every

@@ -20,18 +20,18 @@ static const Option g_option_table[] = {
     {"fk_variant", "DRMB200_FK_VARIANT", 1},     // 0: staging: 1 = TMA bulk copies (default), 0 = cooperative float4 copies
     {"fk_tile", "DRMB200_FK_TILE", 0},           // 1: CTA-tile kernel: configurations per CTA, 64 / 128 / 256; 0 = by batch size
     {"fk_unroll", "DRMB200_FK_UNROLL", 2},       // 2: 0 rolled walk, 1 unrolled register-Jacobian kernel (paths <= 8 links),
-                                                 //    2 = auto: unrolled only for even n_dofs (profiles/r01/v3_sweep_fk_variants.json)
-    {"fk_packed", "DRMB200_FK_PACKED", 1},       // 3: 1 packed FP32x2 arithmetic (default), 0 scalar, 2 two configurations per thread
-    {"rnea_packed", "DRMB200_RNEA_PACKED", 1},   // 4: packed FP32x2 arithmetic in the RNEA kernel
+                                                 //    2 = auto: unrolled only for even n_dofs
+    {"fk_packed", "DRMB200_FK_PACKED", 1},       // 3: 1 f32x2 pair arithmetic (default), 0 scalar, 2 two configurations per thread
+    {"rnea_packed", "DRMB200_RNEA_PACKED", 1},   // 4: f32x2 pair arithmetic in the RNEA kernel
     {"host_fused", "DRMB200_HOST_FUSED", 1},     // 5: drmb200_fk_jacobian_host on page-locked buffers: 1 = one launch whose TMA
                                                  //    copies cross PCIe themselves (default), 0 = staged H2D -> kernel -> D2H
-    {"fk_reserved", "DRMB200_FK_RESERVED", 0},   // 6: unused (was the per-warp pipeline kernel A/B, profiles/r02/v13_lab_fk_launch_per_warp_kernel.json)
+    {"fk_reserved", "DRMB200_FK_RESERVED", 0},   // 6: unused (was the per-warp pipeline kernel A/B)
     {"fk_pdl", "DRMB200_FK_PDL", 0},             // 7: programmatic dependent launch of the FK kernels: 0 off (default);
                                                  //    2 = a launch may run ahead of the FK launches before it on the stream up
                                                  //    to its first global write (the library falls back to an ordinary launch when
                                                  //    an input overlaps an output of the launches still in flight, see
                                                  //    pdl_mode_for_launch in fk_jacobian.cu); 1 = wait before the first global
-                                                 //    read (A/B only: measured slower than 0)
+                                                 //    read (A/B only: slower than 0)
     {"tree_warps", "DRMB200_TREE_WARPS", 0},     // 8: multi-ee tree kernel: warps per CTA (1..4), 0 = auto
     {"tree_grid_cap", "DRMB200_TREE_GRID_CAP", 0},   // 9: multi-ee tree kernel: resident CTAs per SM, 0 = as many as fit
     {"tree_bufs", "DRMB200_TREE_BUFS", 1},       // 10: multi-ee tree kernel: output tiles per warp (1 or 2)
@@ -193,10 +193,9 @@ static int fk_jacobian_host_impl(const drmb200_topology_t* topo, int32_t ee_link
             return DRMB200_OK;
         }
     }
-    // 64 Ki configurations per chunk (14.7 MB per stage for a 7-DoF arm).  Measured on B200/PCIe Gen5:
-    // with 16 Ki chunks a 64 Ki call issues 24 async copies / launches and the ~10 us host cost of each
-    // dominates (185 M cfg/s); with one chunk per 64 Ki it is 214 M cfg/s.  Larger batches pipeline
-    // H2D / kernel / D2H of successive chunks over the three stage streams.
+    // 64 Ki configurations per chunk (14.7 MB per stage for a 7-DoF arm): with 16 Ki chunks a 64 Ki call issues 24
+    // async copies / launches and the host cost of each dominates.  Larger batches pipeline H2D / kernel / D2H of
+    // successive chunks over the three stage streams.
     const int64_t want_chunk = 65536;
     if (g_pipe.device != device || g_pipe.n_dofs != n || g_pipe.chunk != want_chunk) {
         g_pipe.release();

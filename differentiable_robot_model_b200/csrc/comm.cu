@@ -1,11 +1,11 @@
 // comm.cu -- the one exchange step of the data path, fused with the optimiser: SUM all-reduce of the link-parameter gradient
-// over NVLink peer memory + Adam update, in ONE kernel (sm_100a, one process per GPU).
+// over NVLink peer memory + Adam update, in ONE kernel (sm_90a, one process per GPU).
 //
 // The batch of joint configurations shards across GPUs with no data-path collective (SURVEY.md section 8e); the single
 // exception is parameter learning (BASELINE config 5): the gradient of the (fused, flat) link-parameter vector is a batch
 // sum, so the shards' gradients must be added before the optimiser step.  The vector is tiny (91 floats for the 21
-// inertial tensors of the Kuka), so the step is pure latency: an NCCL all-reduce launch + the optimiser launch cost ~28 us
-// per step at 8 GPUs against ~100 us for everything else (profiles/r02/v15_scaling_summary.json).  Here every rank
+// inertial tensors of the Kuka), so the step is pure latency: an NCCL all-reduce launch + the optimiser launch are a
+// large share of the step at 8 GPUs.  Here every rank
 //   1. stores its gradient into a slot of EVERY peer's inbox with plain st.global over NVLink / NVSwitch peer mappings
 //      (cudaIpc handles, exchanged once through torch.distributed), __threadfence_system(), then raises a per-source
 //      sequence flag in each peer's inbox;

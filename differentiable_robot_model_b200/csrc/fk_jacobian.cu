@@ -1,4 +1,4 @@
-// fk_jacobian.cu -- batched forward kinematics + geometric end-effector Jacobian (sm_100a).
+// fk_jacobian.cu -- batched forward kinematics + geometric end-effector Jacobian (sm_90a).
 //
 // Replaces, in ONE launch, the reference's per-link PyTorch graph for
 //   DifferentiableRobotModel.compute_forward_kinematics   (robot_model.py:224-248)
@@ -94,8 +94,8 @@ __device__ __forceinline__ void walk_link(const float* row, const float* qrow, i
     }
 }
 
-// Rolled chain walk with packed FP32x2 arithmetic (FFMA2 / FMUL2): rows 0,1 of R and (p.x, p.y) live in 64-bit register
-// pairs; 35 instead of 54 arithmetic instructions per movable link, same operations in the same order as the scalar walk.
+// Rolled chain walk on f32x2 pairs: rows 0,1 of R and (p.x, p.y) travel as lane pairs; same operations in the same order
+// as the scalar walk.
 // Explicit shared-window addresses (see smem_addr_opaque): table cursor a_tab, this thread's q row a_q and J rows a_jl / a_ja
 // (n4 = 4 n_dofs bytes).  Each path joint parks z_i (its final J_ang column) and z_i x p_i in the thread's rows of the J tile.
 template <bool WITH_JAC>
@@ -143,9 +143,9 @@ __device__ __forceinline__ void jlin_fixup(const PathProgram& prog, int len, uin
     }
 }
 
-// Two configurations per thread: rows `a` and `b` of the tile ride in the two lanes of packed FP32x2 registers, so EVERY
-// arithmetic instruction of the chain walk (R r~, R F~, the axis cross products, Rz) is one FFMA2 / FMUL2 for two
-// configurations, and table loads, loop control and addressing are shared.  Link-table operands are scalar broadcasts.
+// Two configurations per thread: rows `a` and `b` of the tile ride in the two lanes of f32x2 pairs, so every arithmetic
+// operation of the chain walk (R r~, R F~, the axis cross products, Rz) is issued for both configurations back to back,
+// and table loads, loop control and addressing are shared.  Link-table operands are scalar broadcasts.
 // sincos and the quaternion (per-lane branches, integer quadrant logic) run per lane.
 __device__ __forceinline__ f32x2 neg2(f32x2 x) { return mul2(x, bc2(-1.f)); }
 
@@ -308,7 +308,7 @@ fk_jacobian_kernel(const __grid_constant__ PathProgram prog, const FkArgs args) 
 
         if (MAXLEN > 0) {
             V3 zs[MAXLEN > 0 ? MAXLEN : 1], ms[MAXLEN > 0 ? MAXLEN : 1];
-            M3P Rp = identity3p();           // packed FP32x2 state (FFMA2 arithmetic), see drm_common.cuh
+            M3P Rp = identity3p();           // f32x2 pair state, see drm_common.cuh
             f32x2 pp = pk2(0.f, 0.f);
             float p2 = 0.f;
 #pragma unroll
@@ -493,14 +493,14 @@ static int launch_fk(const PathProgram& prog, const FkArgs& args, cudaStream_t s
 
 template <int NDOF, int TILE, bool WITH_JAC>
 static int launch_fk_l(const PathProgram& prog, const FkArgs& args, cudaStream_t stream) {
-    // Rolled vs unrolled (measured, profiles/r01): for odd n (Kuka, 7) the rolled kernel wins (21.9 vs 19.8 G cfg/s).
-    // For even n the per-thread J rows have even strides -> 16-way bank conflicts on every J access; the unrolled
-    // kernel touches the J tile once per column instead of three times and wins (Allegro, n = 16: 9.8 vs 6.3 G cfg/s).
+    // Rolled vs unrolled: for odd n (Kuka, 7) the rolled kernel wins.  For even n the per-thread J rows have even
+    // strides -> 16-way bank conflicts on every J access; the unrolled kernel touches the J tile once per column instead
+    // of three times and wins (Allegro, n = 16).  Chosen by sweeps before the H100 port; not re-measured on the H100.
     const int opt = get_option(2);                     // 0 rolled, 1 unrolled, 2 auto
     const bool unrolled = prog.len <= 8 && (opt == 1 || (opt != 0 && (prog.n_dofs % 2) == 0));
     if (unrolled) return launch_fk<NDOF, TILE, WITH_JAC, 8>(prog, args, stream);
-    // rolled walk: packed FP32x2 arithmetic (FFMA2) unless switched off for A/B measurements
-    // fk_packed = 2: two configurations per thread in the two FP32x2 lanes (A/B candidate, see pair_walk)
+    // rolled walk: f32x2 pair arithmetic unless switched off for A/B measurements
+    // fk_packed = 2: two configurations per thread in the two f32x2 lanes (A/B candidate, see pair_walk)
     const int packed = get_option(3);
     if (packed == 2) return launch_fk<NDOF, TILE, WITH_JAC, -2>(prog, args, stream);
     return packed != 0 ? launch_fk<NDOF, TILE, WITH_JAC, -1>(prog, args, stream)
@@ -533,10 +533,21 @@ static int g_log_clock = 0;
 
 static bool overlaps(const PdlRange& a, const PdlRange& b) { return a.lo < b.hi && b.lo < a.hi; }
 
-// mode the launch may use (0 or the requested one) + log its output ranges; smem_share = f above
-int pdl_decide(cudaStream_t stream, const PdlRange* ins, int n_ins, const PdlRange outs[4], double smem_share) {
+int device_sm_count() {
+    static int sms_by_dev[64] = {0};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    int& sms = sms_by_dev[dev & 63];
+    if (sms == 0 && (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)) { cudaGetLastError(); sms = 132; }
+    return sms;
+}
+
+// mode the launch may use (0 or the requested one) + log its output ranges; f above = grid_smem_bytes over the
+// device's shared memory (227 KB per SM)
+int pdl_decide(cudaStream_t stream, const PdlRange* ins, int n_ins, const PdlRange outs[4], double grid_smem_bytes) {
     int mode = get_option(7);
     if (mode < 0 || mode > 2) mode = 0;
+    const double smem_share = grid_smem_bytes / ((double)device_sm_count() * 227.0 * 1024.0);
     int dev = 0;
     cudaGetDevice(&dev);
     std::lock_guard<std::mutex> lock(g_log_mu);
@@ -571,7 +582,7 @@ static int pdl_mode_for_launch(const PathProgram& prog, const FkArgs& args, int 
     const PdlRange ins[2] = {pdl_range(args.q, B * 4 * n), pdl_range(args.table, (uintptr_t)n_links * DRMB200_TABLE_STRIDE * 4)};
     // share of the GPU's shared memory this grid takes (the residency bound above)
     const double smem_per_config = 4.0 * (n + 7 + (args.jlin ? 6 * n : 0));
-    return pdl_decide(stream, ins, 2, outs, smem_per_config * (double)args.batch / (148.0 * 227.0 * 1024.0));
+    return pdl_decide(stream, ins, 2, outs, smem_per_config * (double)args.batch);
 }
 
 int fk_jacobian_device(const drmb200_topology_t* topo, int32_t ee_link, const float* table, const float* q,
@@ -609,25 +620,24 @@ int fk_jacobian_device(const drmb200_topology_t* topo, int32_t ee_link, const fl
     args.use_bulk = get_option(0) != 0;
     const bool with_jac = jlin != nullptr;
     // n_dofs % 4 == 0 (Allegro, n = 16): the per-lane rows of this kernel's natural-layout tiles are 16-way bank
-    // conflicts; the tree-walk kernel (fk_tree.cu) assembles 16-byte column chunks instead.  Measured, one Allegro
-    // fingertip (profiles/r02): 2^21 per launch 0.78 of the HBM roofline there vs 0.71 here (unrolled variant); 32 768 per
-    // launch 0.57 there vs 0.63 here -- so large batches are routed to the tree kernel, small ones stay.
+    // conflicts; the tree-walk kernel (fk_tree.cu) assembles 16-byte column chunks instead.  For one Allegro fingertip the
+    // tree kernel was the faster of the two at 2^21 per launch and the slower at 32 768 -- so large batches are routed to
+    // the tree kernel, small ones stay (chosen before the H100 port; not re-measured on the H100).
     if ((prog.n_dofs & 3) == 0 && prog.n_dofs > 0 && batch >= 262144 && get_option(2) == 2)
         return fk_jacobian_multi_device(topo, 1, &ee_link, table, q, batch, pos, quat, jlin, jang, stream);
     args.pdl = pdl_mode_for_launch(prog, args, topo->n_links, stream);
 
 
-    // Tile size, from the measured sweep (profiles/r01/v3_sweep_fk_variants.json, Kuka, rolled kernel):
-    //   2^22 per launch:   tile 64 -> 21.99 G cfg/s, 128 -> 20.96, 256 -> 16.66   (shared memory, 32 n + 28 bytes
-    //                      per configuration, is the occupancy limiter: smaller tiles pack SMs tighter)
-    //   65 536 per launch, 4 launches in flight: tile 128 -> 3.19 us, 64 -> 3.29 us, 256 -> 4.01 us
-    int tile = get_option(1);
-    //   16-DoF Allegro hand, 2^21 per launch: tile 128 -> 9.8 G cfg/s, tile 64 -> 7.0 (even row strides: 16-way
-    //                      bank conflicts hurt the narrower tile more), so wide rows keep 128
+    // Tile size (Kuka, rolled kernel; chosen by sweeps before the H100 port, not re-measured on the H100):
+    //   large batches: tile 64 (shared memory, 32 n + 28 bytes per configuration, is the occupancy limiter: smaller
+    //                  tiles pack SMs tighter); 256 is slowest
+    //   batches up to 1 Ki per SM without programmatic dependent launch: tile 128 (fewer CTAs, shorter sub-wave ramp)
+    //   wide rows (n > 8, e.g. the 16-DoF Allegro hand): 128 (even row strides: bank conflicts hurt the narrower tile more)
     //   with programmatic dependent launch (fk_pdl 2) consecutive launches overlap and the sub-wave ramp no longer
-    //   matters: tile 64 -> 2.85 us per stream-ordered 65 536 launch, tile 128 -> 3.41 us (profiles/r02/v13_lab_fk_launch_pdl.json)
+    //   matters: tile 64
+    int tile = get_option(1);
     if (tile != 64 && tile != 128 && tile != 256)
-        tile = (prog.n_dofs > 8 || (batch <= 148 * 1024 && args.pdl != 2)) ? 128 : 64;
+        tile = (prog.n_dofs > 8 || (batch <= (int64_t)device_sm_count() * 1024 && args.pdl != 2)) ? 128 : 64;
     switch (prog.n_dofs) {
         case 2: return launch_fk_t<2>(tile, with_jac, prog, args, stream);
         case 7: return launch_fk_t<7>(tile, with_jac, prog, args, stream);

@@ -1,4 +1,4 @@
-// fk_tree.cu -- FK + geometric Jacobians of SEVERAL end-effector links in ONE walk of the kinematic tree (sm_100a).
+// fk_tree.cu -- FK + geometric Jacobians of SEVERAL end-effector links in ONE walk of the kinematic tree (sm_90a).
 //
 // The reference computes one end effector per call: compute_endeffector_jacobian (robot_model.py:627-667) runs the whole
 // update_kinematic_state pass (robot_model.py:140-195) and then walks ee -> root.  A hand (Allegro: four fingertips off
@@ -9,7 +9,7 @@
 //   * one WARP = one pipeline over tiles of 32 configurations (one configuration per lane, no CTA-wide barrier after the
 //     table has been staged); persistent grid, the q tile of the next tile is in flight (TMA bulk load, own mbarrier)
 //     while the current one is walked;
-//   * the state (R, p) of the previous link stays in registers (packed FP32x2 arithmetic as in fk_jacobian.cu), branch
+//   * the state (R, p) of the previous link stays in registers (f32x2 pair arithmetic as in fk_jacobian.cu), branch
 //     points spill it to slot-major shared memory; every movable link parks its joint axis z_i and z_i x p_i in a
 //     slot-major scratch indexed by its DEPTH among the movable links of the path (siblings reuse the slots);
 //   * at an end effector the Jacobian columns of its path are assembled from the scratch (J_lin = z_i x p_ee - z_i x p_i,
@@ -422,15 +422,6 @@ static int build_multi_program(const drmb200_topology_t* topo, int32_t n_ee, con
     return DRMB200_OK;
 }
 
-static int mt_sm_count() {
-    static int sms_by_dev[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    int& sms = sms_by_dev[dev & 63];
-    if (sms == 0 && (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)) { cudaGetLastError(); sms = 148; }
-    return sms;
-}
-
 template <int NDOF, bool CHUNK, bool WITH_JAC>
 static int launch_fk_tree(const MultiProgram& prog, const MtArgs& args, cudaStream_t stream) {
     const MtWarpLayout L(prog.n_dofs, prog.n_jslots, prog.n_state_slots, WITH_JAC, args.nbuf);
@@ -439,7 +430,7 @@ static int launch_fk_tree(const MultiProgram& prog, const MtArgs& args, cudaStre
     const size_t cap = 227 * 1024 - 256;
     if (tab_bytes + warp_bytes > cap) { set_error("multi-ee FK needs %zu B of shared memory per warp (> 227 KB)", tab_bytes + warp_bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (args.batch + 31) >> 5;
-    const int sms = mt_sm_count();
+    const int sms = device_sm_count();
     // warps per CTA: 2 keeps the CTA small enough that several fit per SM and the tiles of a small batch spread evenly
     int warps = get_option(8);
     if (warps < 1 || warps > MT_WARPS_MAX) warps = 2;
@@ -469,7 +460,7 @@ static int launch_fk_tree(const MultiProgram& prog, const MtArgs& args, cudaStre
                                   pdl_range(args.jang, Bn * 12 * n)};
         const PdlRange ins[2] = {pdl_range(args.q, (uintptr_t)args.batch * 4 * n),
                                  pdl_range(args.table, (uintptr_t)DRMB200_MAX_LINKS * DRMB200_TABLE_STRIDE * 4)};
-        const int mode = pdl_decide(stream, ins, 2, outs, (double)ctas * (double)smem_bytes / (148.0 * 227.0 * 1024.0));
+        const int mode = pdl_decide(stream, ins, 2, outs, (double)ctas * (double)smem_bytes);
         largs.pdl = mode == 2 ? 2 : 0;
     }
     cudaLaunchConfig_t cfg = {};

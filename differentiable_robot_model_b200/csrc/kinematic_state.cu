@@ -1,4 +1,4 @@
-// kinematic_state.cu -- world pose and body-frame spatial velocity of EVERY link in one launch (sm_100a).
+// kinematic_state.cu -- world pose and body-frame spatial velocity of EVERY link in one launch (sm_90a).
 //
 // Replaces DifferentiableRobotModel.update_kinematic_state (robot_model.py:140-195) -- the pass that leaves
 // `_bodies[i].pose` / `_bodies[i].vel` behind in the reference -- and, with the quaternion output enabled,

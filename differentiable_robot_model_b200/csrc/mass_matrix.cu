@@ -1,4 +1,4 @@
-// mass_matrix.cu -- batched joint-space inertia matrix H(q) [B, n, n] in ONE launch (sm_100a).
+// mass_matrix.cu -- batched joint-space inertia matrix H(q) [B, n, n] in ONE launch (sm_90a).
 //
 // Replaces DifferentiableRobotModel.compute_lagrangian_inertia_matrix (robot_model.py:403-450), which evaluates
 // compute_inverse_dynamics n + 1 times (column j = ID(q, 0, e_j) - ID(q, 0, 0), every evaluation a full walk of the
@@ -9,7 +9,7 @@
 //     column j:  al_i = E al_p + e_z [i = j],  a_i = E (a_p + al_p x r)          (zero above the subtree of j)
 //                f_i = m a_i - mc x al_i,  n_i = Io al_i + mc x a_i             (no velocity terms)
 //                leaves -> root:  f_p += M f_i,  n_p += r x (M f_i) + M n_i,  H[dof(i), j] = n_i.z
-// The (al | a) pair goes through E = Rz^T F~^T as packed FP32x2 (drm_common.cuh).  H is staged in shared memory in
+// The (al | a) pair goes through E = Rz^T F~^T as f32x2 pair (drm_common.cuh).  H is staged in shared memory in
 // its global row-major layout and leaves as one TMA bulk store per tile.
 //
 // Algorithmic HBM bytes per configuration: 4n in + 4n^2 out (224 B at n = 7); about 1 k instructions per column and

@@ -1,4 +1,4 @@
-// rnea.cu -- batched recursive Newton-Euler inverse dynamics (sm_100a).
+// rnea.cu -- batched recursive Newton-Euler inverse dynamics (sm_90a).
 //
 // Replaces, in ONE launch, DifferentiableRobotModel.compute_inverse_dynamics (robot_model.py:306-375):
 // update_kinematic_state (robot_model.py:140-195, velocities), update_joint_acc (rigid_body.py:159-165),
@@ -77,9 +77,9 @@ struct RneaSmemLayout {
 
 // DUMP additionally writes the per-link state the reference leaves in `_bodies[i].vel / .acc / .force`
 // (robot_model.py:183-193, 262-301), un-permuted to the natural link frames, link-major / component-major (coalesced).
-// (A per-warp pipeline version of this kernel -- persistent grid, no CTA barrier, like fk_tree.cu -- was measured at
-// 10.2 G cfg/s against 11.3 G for this CTA-tile form on the Panda: the kernel is issue-bound and the extra loop /
-// addressing instructions cost more than the barrier stalls they remove.)
+// (A per-warp pipeline version of this kernel -- persistent grid, no CTA barrier, like fk_tree.cu -- was slower than this
+// CTA-tile form on the Panda: the kernel is issue-bound and the extra loop / addressing instructions cost more than the
+// barrier stalls they remove.)
 template <int T, bool PACKED, bool DUMP, bool FOLD>
 __global__ void __launch_bounds__(T)
 rnea_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const RneaArgs args) {
@@ -152,9 +152,9 @@ rnea_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ Fo
         };
 
         // ---- pass 1: root -> leaves, motion state + body wrench ------------------------------------
-        // Packed FP32x2 arithmetic (drm_common.cuh): the velocity-level and the acceleration-level quantities obey the
+        // f32x2 pair arithmetic (drm_common.cuh): the velocity-level and the acceleration-level quantities obey the
         // same linear maps, so they travel as PAIRS -- W = (w | al), V = (v | a) -- and every 3x3 product, cross
-        // product with r and spatial-inertia product is one FFMA2 per two scalar FMAs.
+        // product with r and spatial-inertia product is written once for both.
         const V3 zero = v3(0.f, 0.f, 0.f);
         V3P W = pk3(zero, zero), V = W;                     // state of the previously processed link
         if (DUMP) {                                         // the root: zero velocity, base acceleration, wrench accumulator
@@ -464,8 +464,8 @@ const CachedPrograms* cached_programs(const drmb200_topology_t* topo, int* rc_ou
 }
 
 // The folded canonical table of a link table, once, for callers whose table does not change between launches (constant
-// models): staging it per CTA costs 13-15 % of the inverse-dynamics kernel (measured by skipping it: 15.7 against 13.6 G cfg/s
-// at 65 536 per launch), a plain copy of n_red x 28 floats costs nothing.  Output: [n_red, 28] canonical rows (row 0 unused).
+// models): folding it while staging costs every CTA a noticeable share of the inverse-dynamics kernel, a plain copy of
+// n_red x 28 floats costs nothing.  Output: [n_red, 28] canonical rows (row 0 unused).
 __global__ void __launch_bounds__(64)
 fold_table_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold,
                   const float* __restrict__ table, float* __restrict__ folded) {
@@ -535,18 +535,18 @@ int inverse_dynamics_device(const drmb200_topology_t* topo, const float* table, 
     // "rnea_fold" (default on): walk only the movable links, fixed links folded into their movable ancestors at staging time
     const bool fold = cp->foldable && get_option(11) != 0;
     const TreeProgram* prog = fold ? &cp->red : &cp->full;
-    // tile: 128 amortises the table staging (heavier since it folds the fixed links) over twice the configurations:
-    // 13.4 against 11.9 G cfg/s at 65 536 per launch, 13.0 against 11.5 at 2^21 (Panda, profiles/r02); 64 only for batches
-    // that would leave SMs without a CTA, and for models whose 128-row footprint is too big
+    // tile: 128 amortises the table staging (heavier since it folds the fixed links) over twice the configurations
+    // (chosen by a Panda sweep before the H100 port; not re-measured on the H100); 64 only for batches that would leave
+    // SMs without a CTA, and for models whose 128-row footprint is too big
     int tile = (batch < 32768) ? 64 : 128;
-    if (get_option(12) == 64 || get_option(12) == 128) tile = get_option(12);      // 256 was measured too: 11.7 G cfg/s
+    if (get_option(12) == 64 || get_option(12) == 128) tile = get_option(12);      // 256 lost that sweep too
     if ((size_t)RneaSmemLayout(128, prog->n_dofs, prog->n_links, prog->n_slots).total_floats * sizeof(float) > 110 * 1024) tile = 64;
     RneaArgs args;
     args.table = table; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau; args.batch = batch; args.flags = flags;
     args.vels = args.accs = args.forces = nullptr;
     auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
     args.aligned = (al16(q) && al16(qd) && al16(qdd) && al16(tau)) ? 1 : 0;
-    const bool packed = get_option(4) != 0;             // "rnea_packed": FP32x2 arithmetic (default) vs scalar, for A/B runs
+    const bool packed = get_option(4) != 0;             // "rnea_packed": f32x2 pair arithmetic (default) vs scalar, for A/B runs
     if (fold) {
         if (tile == 64) return packed ? launch_rnea<64, true, false, true>(*prog, cp->fold, args, stream) : launch_rnea<64, false, false, true>(*prog, cp->fold, args, stream);
         return packed ? launch_rnea<128, true, false, true>(*prog, cp->fold, args, stream) : launch_rnea<128, false, false, true>(*prog, cp->fold, args, stream);

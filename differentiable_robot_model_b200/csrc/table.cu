@@ -1,4 +1,4 @@
-// table.cu -- link-parameter rows -> link table, forward and analytic backward (sm_100a).
+// table.cu -- link-parameter rows -> link table, forward and analytic backward (sm_90a).
 //
 // The host gathers, per link, the raw parameters the reference keeps in per-link modules
 //   raw[i] = [ rpy(3) | trans(3) | mass | com(3) | inertia_mat(9, at the COM) | damping ]     (20 floats)
@@ -7,9 +7,8 @@
 //   F  = Rz(yaw) Ry(pitch) Rx(roll)                      rigid_body.py:138-143
 //   Io = I_c + m (|c|^2 I - c c^T)   (= I_c + m S(c)S(c)^T), mc = m c    spatial_vector_algebra.py:323-327
 // With learnable link parameters the table must be rebuilt -- differentiably -- on every call; done with
-// torch ops that is ~60 tiny launches forward and ~100 autograd nodes backward (0.8 ms + 0.8 ms per training
-// step, profiles/r01/v3_train_step_profile.json), four times the cost of the RNEA forward + backward kernels
-// themselves.  One thread per link; n_links <= 64.
+// torch ops that is ~60 tiny launches forward and ~100 autograd nodes backward per training step, several times
+// the cost of the RNEA forward + backward kernels themselves.  One thread per link; n_links <= 64.
 #include "drm_common.cuh"
 
 namespace drm {

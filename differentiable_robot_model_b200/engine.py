@@ -2,7 +2,7 @@
 ctypes binding of the C-ABI library + torch.autograd plumbing
 ================================================================
 ``libdrm_b200.so`` (``csrc/``, declared in ``include/drm_b200.h``) is the product: hand-written
-sm_100a kernels behind an ``extern "C"`` interface with plain pointers.  This module loads it with
+sm_90a kernels behind an ``extern "C"`` interface with plain pointers.  This module loads it with
 ctypes (no torch types cross the boundary -- only ``tensor.data_ptr()`` and the raw handle of the
 current CUDA stream) and wraps the forward / backward entry points in ``torch.autograd.Function``s so
 that the reference's parameter-learning examples keep training.
@@ -106,7 +106,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(_LIB_PATH):
             raise RuntimeError(
-                f"{_LIB_PATH} not found: the B200 CUDA engine has not been built "
+                f"{_LIB_PATH} not found: the CUDA engine has not been built "
                 "(run `python -c 'import __graft_entry__ as g; g.build()'` or `make -C "
                 "differentiable_robot_model_b200/csrc`). There is no CPU fallback."
             )
@@ -146,7 +146,7 @@ _NO_GUARD = _NoGuard()
 
 def _on(device):
     """Context that makes `device` current for a launch.  A no-op object when it already is (the usual case): entering
-    torch.cuda.device() costs ~3 us per call, a third of a batch-1 call's host time (profiles/r02/v15_latency_batch1.json)."""
+    torch.cuda.device() costs microseconds of host time per call, a large share of a batch-1 call."""
     if device.index is None or device.index == torch.cuda.current_device():
         return _NO_GUARD
     return torch.cuda.device(device)
@@ -159,7 +159,7 @@ def _require_cuda(*tensors):
             continue
         if not t.is_cuda:
             raise RuntimeError(
-                "the B200 engine computes on CUDA tensors only (got a tensor on "
+                "the engine computes on CUDA tensors only (got a tensor on "
                 f"{t.device}); there is no CPU fallback"
             )
         if t.dtype != torch.float32:

@@ -1,5 +1,5 @@
 """
-Differentiable robot model -- B200 engine behind the reference's API
+Differentiable robot model -- CUDA engine behind the reference's API
 =====================================================================
 Drop-in for ``differentiable_robot_model.robot_model`` (reference ``robot_model.py``): same class and
 wrapper names, constructor, method names, keyword arguments, return-tuple order, squeeze behaviour
@@ -8,7 +8,7 @@ reference walks a Python list of per-link ``nn.Module``s issuing dozens of tiny 
 per link (``robot_model.py:173-193, 262-301``); here a call is
 
     argument checks -> link table (cached, or rebuilt differentiably when parameters are learnable)
-    -> ONE hand-written sm_100a kernel through the C ABI (``engine.py`` / ``include/drm_b200.h``)
+    -> ONE hand-written sm_90a kernel through the C ABI (``engine.py`` / ``include/drm_b200.h``)
 
 on the caller's current CUDA stream, with analytic backward kernels registered through
 ``torch.autograd.Function`` so the parameter-learning examples still train.
@@ -81,7 +81,7 @@ def tensor_check(function):
 
 
 class DifferentiableRobotModel(torch.nn.Module):
-    """Batched rigid-body kinematics / dynamics of a URDF robot on one B200 GPU."""
+    """Batched rigid-body kinematics / dynamics of a URDF robot on one GPU (H100, sm_90a)."""
 
     def __init__(self, urdf_path: str, name="", device=None):
         super().__init__()

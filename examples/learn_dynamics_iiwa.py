@@ -1,4 +1,4 @@
-"""Identify link-1 mass / inertia and the link-2 joint origin of a Kuka iiwa from joint torques (B200 engine).
+"""Identify link-1 mass / inertia and the link-2 joint origin of a Kuka iiwa from joint torques (CUDA engine).
 
 The experiment of the reference's ``examples/learn_dynamics_iiwa.py`` (entry point ``run(n_epochs, n_data, device)``,
 :49): ground-truth torques along a sine motion, a copy of the model with three learnable link parameters, Adam on the

@@ -1,4 +1,4 @@
-"""Identify link-1 mass / centre of mass / inertia of a Kuka iiwa from joint accelerations (B200 engine).
+"""Identify link-1 mass / centre of mass / inertia of a Kuka iiwa from joint accelerations (CUDA engine).
 
 The experiment of the reference's ``examples/learn_forward_dynamics_iiwa.py`` (``run(n_epochs, n_data, device)``, :50).
 Every ``compute_forward_dynamics`` call is ONE articulated-body kernel launch and ``backward()`` its analytic adjoint

@@ -1,4 +1,4 @@
-"""Recover the joint origin (trans, rot_angles) of Kuka iiwa link 1 from end-effector positions (B200 engine).
+"""Recover the joint origin (trans, rot_angles) of Kuka iiwa link 1 from end-effector positions (CUDA engine).
 
 The experiment of the reference's ``examples/learn_kinematics_of_iiwa.py`` (``run(n_epochs, n_data, device)``, :26):
 one FK kernel launch forward, the analytic FK adjoint kernel backward.

@@ -1,5 +1,5 @@
 """Recover both joint origins of the planar 2-link toy robot from end-effector positions, freezing one of them for a
-while on the way (B200 engine).
+while on the way (CUDA engine).
 
 The experiment of the reference's ``examples/learn_kinematics_of_toy.py`` (``run(n_epochs, n_data, device)``, :27),
 including its freeze at iteration 10 / unfreeze at iteration 100.

@@ -1,5 +1,5 @@
 /*
- * drm_b200.h -- C ABI of the B200-native batched rigid-body kinematics/dynamics engine.
+ * drm_b200.h -- C ABI of the batched rigid-body kinematics/dynamics engine (CUDA, sm_90a).
  *
  * This is the drop-in boundary for the hot path of facebookresearch/differentiable-robot-model
  * (reference paths below are relative to /root/reference):
@@ -90,9 +90,9 @@ int64_t drmb200_launch_count(void);        /* kernels launched by this library s
  *   "fk_variant": 1 = TMA bulk-copy staging (default), 0 = cooperative float4 staging;
  *   "fk_tile":    configurations per CTA of the FK kernel, 64 / 128 / 256, 0 = chosen from the batch size (default);
  *   "fk_unroll":  0 = rolled chain walk, 1 = unrolled register-Jacobian kernel (paths <= 8 links), 2 = auto (default);
- *   "fk_packed":  1 = packed FP32x2 arithmetic (FFMA2) in the rolled chain walk (default), 0 = scalar FFMA,
- *                 2 = two configurations per thread in the two FP32x2 lanes (measured slower; kept for A/B);
- *   "rnea_packed": 1 = packed FP32x2 arithmetic in the inverse-dynamics kernel (default), 0 = scalar FFMA;
+ *   "fk_packed":  1 = f32x2 pair arithmetic in the rolled chain walk (default), 0 = scalar FMA,
+ *                 2 = two configurations per thread in the two f32x2 lanes (kept for A/B);
+ *   "rnea_packed": 1 = f32x2 pair arithmetic in the inverse-dynamics kernel (default), 0 = scalar FMA;
  *   "rnea_fold":  1 = the inverse-dynamics kernel walks only the movable links, links behind fixed joints are folded into
  *                 their nearest movable ancestor while the table is staged (default), 0 = one step per link like the reference;
  *   "rnea_bwd_chain": drmb200_inverse_dynamics_backward on robots whose links form one serial chain (every link's parent is
@@ -105,8 +105,8 @@ int64_t drmb200_launch_count(void);        /* kernels launched by this library s
  *                 WRITE.  Results are identical to mode 0 for every legal call sequence: the library tracks the output
  *                 ranges of the FK launches that can still be in flight on the stream and issues an ordinary launch
  *                 whenever q or the table of the new launch overlaps one of them (and for batches too small to bound
- *                 how many launches can be in flight).  Measured: 2.85 us instead of 6.8 us per stream-ordered launch
- *                 of 65 536 Kuka configurations.  1: wait before the first global read (A/B only, slower than 0). */
+ *                 how many launches can be in flight).  Measured on an H100 SXM (400 W power limit): 5.96 us instead of
+ *                 9.11 us per stream-ordered launch of 65 536 Kuka configurations.  1: wait before the first global read (A/B only, slower than 0). */
 int drmb200_set_option(const char* name, int value);
 int drmb200_get_option(const char* name, int* value);   /* the value in effect (environment / default / last set) */
 

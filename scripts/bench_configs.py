@@ -22,7 +22,7 @@ from differentiable_robot_model_b200.rigid_body_params import UnconstrainedScala
 from oracle import drm_oracle as O  # noqa: E402
 
 DEV = torch.device("cuda", 0)
-PEAK = 6567.4
+PEAK = 3350.0                 # H100 SXM data-sheet HBM3 bandwidth (GB/s) unless MEASURED_PEAKS.json gives a measured one
 try:
     PEAK = float(json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:

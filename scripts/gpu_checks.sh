@@ -1,5 +1,5 @@
 #!/bin/bash
-# Run on the B200 box via:  gpurun --timeout 2400 -- 'bash scripts/gpu_checks.sh [quick]'
+# Run from the repository root on an H100:  bash scripts/gpu_checks.sh [quick]
 # Parity tests, smoke, bench (+ reference arm), ncu launch list and --set full captures, secondary configs.
 set -u
 mkdir -p gpurun_out

@@ -82,7 +82,7 @@ def main():
             stream.synchronize()
             ms = e0.elapsed_time(e1) / 10
             row["big_us"] = ms * 1e3
-            row["big_frac_of_6567"] = big * BYTES / ms / 1e6 / 6567.4
+            row["big_frac_of_3350"] = big * BYTES / ms / 1e6 / 3350.0     # H100 SXM data-sheet HBM3 GB/s
             # isolated launches after an L2 flush
             iso = []
             for i in range(12):
@@ -133,7 +133,7 @@ def main():
                 for o in outs:
                     for t in o:
                         t.zero_()
-                row[f"{key}_frac_of_6567"] = small * BYTES / us / 1e3 / 6567.4
+                row[f"{key}_frac_of_3350"] = small * BYTES / us / 1e3 / 3350.0
                 del g
         rows.append(row)
         print(json.dumps(row), file=sys.stderr, flush=True)

@@ -29,7 +29,7 @@ URDFS = {
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
     # the CPU oracle issues thousands of tiny torch ops: on a 128-core host the default intra-op
     # thread count makes each of them slower, not faster
     import torch

@@ -1,4 +1,4 @@
-"""GPU: batches beyond the small-batch tile switch (148 Ki rows) take the wide-tile kernel instantiations; every row must
+"""GPU: batches beyond the small-batch tile switch (1 Ki rows per SM, 132 Ki on an H100) take the wide-tile kernel instantiations; every row must
 be bit-identical to the same row computed in a small batch (narrow tiles), for FK+Jacobian and RNEA."""
 import pytest
 import torch
