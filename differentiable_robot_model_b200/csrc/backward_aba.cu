@@ -44,6 +44,7 @@ struct AbaBwdArgs {
     int64_t batch;
     uint32_t flags;
     int32_t vec_ok;
+    int32_t accumulate;                // add to the per-CTA partial tables instead of overwriting them
 };
 
 struct AbaBwdSmem {
@@ -553,7 +554,8 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
             const int p = prog.parent[l];
             int src;
             const float sg = canon_map(e, p >= 0 ? (int)prog.axis[p] : 0, prog.axis[l], src);
-            out[l * DRMB200_TABLE_STRIDE + src] = sg * s_acc[i];
+            const float v = sg * s_acc[i];
+            out[l * DRMB200_TABLE_STRIDE + src] = args.accumulate ? out[l * DRMB200_TABLE_STRIDE + src] + v : v;
         }
     }
 }
@@ -567,10 +569,13 @@ int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t* topo
     return table_grad_workspace_bytes(topo, batch) + grid * (topo->n_links - 1) * IA_FLOATS * 32 * (int64_t)sizeof(float);
 }
 
+// accumulate_partials / reduce: a caller that runs the adjoint several times on batches of the same size (the steps of a
+// rollout, rollout.cu) can sum the per-CTA partial tables of all calls in the workspace and reduce them into table_grad once,
+// with the last call; the default (false, true) is one self-contained adjoint.
 int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                                      const float* f, int64_t batch, uint32_t flags, const float* g_qdd,
                                      float* q_grad, float* qd_grad, float* f_grad, float* table_grad, void* workspace,
-                                     cudaStream_t stream) {
+                                     cudaStream_t stream, bool accumulate_partials, bool reduce) {
     TreeProgram prog;
     int rc = build_tree_program(topo, &prog);
     if (rc != DRMB200_OK) return rc;
@@ -586,6 +591,7 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     args.partials = static_cast<float*>(workspace);
     args.scratch = reinterpret_cast<float*>(static_cast<char*>(workspace) + table_grad_workspace_bytes(topo, batch));
     args.batch = batch; args.flags = flags;
+    args.accumulate = accumulate_partials ? 1 : 0;
     auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
     args.vec_ok = (al16(q) && al16(qd) && al16(f) && al16(g_qdd) && al16(q_grad) && al16(qd_grad) && al16(f_grad)) ? 1 : 0;
 
@@ -608,7 +614,15 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("aba backward launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
     count_launch();
-    return need_table ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
+    return need_table && reduce ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
+}
+
+int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
+                                     const float* f, int64_t batch, uint32_t flags, const float* g_qdd,
+                                     float* q_grad, float* qd_grad, float* f_grad, float* table_grad, void* workspace,
+                                     cudaStream_t stream) {
+    return forward_dynamics_backward_device(topo, table, q, qd, f, batch, flags, g_qdd, q_grad, qd_grad, f_grad, table_grad,
+                                            workspace, stream, false, true);
 }
 
 }  // namespace drm

@@ -96,6 +96,12 @@ int forward_dynamics_device(const drmb200_topology_t*, const float*, const float
                             int64_t, uint32_t, float*, cudaStream_t);
 int forward_dynamics_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*,
                                      int64_t, uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t);
+int forward_dynamics_rollout_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
+                                    int32_t, float, uint32_t, float*, float*, float*, cudaStream_t);
+int64_t forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
+int forward_dynamics_rollout_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*,
+                                             int64_t, int32_t, float, uint32_t, const float*, const float*, const float*,
+                                             const float*, const float*, float*, float*, float*, float*, void*, cudaStream_t);
 int64_t table_grad_workspace_bytes(const drmb200_topology_t*, int64_t);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 int mass_matrix_device(const drmb200_topology_t*, const float*, const float*, int64_t, float*, cudaStream_t);
@@ -348,6 +354,27 @@ int drmb200_forward_dynamics_backward(const drmb200_topology_t* topo, const floa
                                       float* table_grad, void* workspace, void* cuda_stream) {
     return drm::forward_dynamics_backward_device(topo, table, q, qd, f, batch, flags, g_qdd, q_grad, qd_grad, f_grad,
                                                  table_grad, workspace, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_forward_dynamics_rollout(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
+                                     const float* f, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q,
+                                     float* qd, float* qdd, void* cuda_stream) {
+    return drm::forward_dynamics_rollout_device(topo, table, q0, qd0, f, batch, n_steps, dt, flags, q, qd, qdd,
+                                                static_cast<cudaStream_t>(cuda_stream));
+}
+
+int64_t drmb200_forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
+    return drm::forward_dynamics_rollout_backward_workspace_bytes(topo, batch);
+}
+
+int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, const float* table, const float* q0,
+                                              const float* qd0, const float* f, int64_t batch, int32_t n_steps, float dt,
+                                              uint32_t flags, const float* q, const float* qd, const float* g_q,
+                                              const float* g_qd, const float* g_qdd, float* q0_grad, float* qd0_grad,
+                                              float* f_grad, float* table_grad, void* workspace, void* cuda_stream) {
+    return drm::forward_dynamics_rollout_backward_device(topo, table, q0, qd0, f, batch, n_steps, dt, flags, q, qd, g_q, g_qd,
+                                                         g_qdd, q0_grad, qd0_grad, f_grad, table_grad, workspace,
+                                                         static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_kinematic_state(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -69,6 +69,15 @@ _SIGNATURES = {
                                                          _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p,
                                                          _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                          ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_forward_dynamics_rollout": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                        ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_uint32,
+                                                        _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
+    "drmb200_forward_dynamics_rollout_backward_workspace_bytes": (ctypes.c_int64, [ctypes.POINTER(Topology), ctypes.c_int64]),
+    "drmb200_forward_dynamics_rollout_backward": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
+                                                                 _c_float_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_float,
+                                                                 ctypes.c_uint32, _c_float_p, _c_float_p, _c_float_p,
+                                                                 _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                                 _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
     "drmb200_kinematic_state": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
                                                _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table": (ctypes.c_int, [_c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_void_p]),
@@ -274,6 +283,23 @@ def forward_dynamics_raw(topo, table, q, qd, f, flags, out=None, folded=None):
                                                 flags, _ptr(qdd), _stream())
     _check(rc, "drmb200_forward_dynamics")
     return qdd
+
+
+def forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags, want_qdd=True):
+    """(q, qd, qdd) [T, B, n] of T semi-implicit Euler steps over the articulated-body algorithm, one launch
+    (drmb200_forward_dynamics_rollout); qdd is None unless want_qdd."""
+    _require_cuda(table, q0, qd0, f)
+    q0, qd0, f = q0.contiguous(), qd0.contiguous(), f.contiguous()
+    T, B, n = f.shape
+    dev = q0.device
+    q = torch.empty((T, B, n), device=dev, dtype=torch.float32)
+    qd = torch.empty((T, B, n), device=dev, dtype=torch.float32)
+    qdd = torch.empty((T, B, n), device=dev, dtype=torch.float32) if want_qdd else None
+    with _on(dev):
+        rc = lib().drmb200_forward_dynamics_rollout(ctypes.byref(topo), _ptr(table), _ptr(q0), _ptr(qd0), _ptr(f), B, T,
+                                                    ctypes.c_float(dt), flags, _ptr(q), _ptr(qd), _ptr(qdd), _stream())
+    _check(rc, "drmb200_forward_dynamics_rollout")
+    return q, qd, qdd
 
 
 def kinematic_state_raw(topo, table, q, qd=None, want_poses=True, want_quats=False):
@@ -577,6 +603,41 @@ class ForwardDynamicsFunction(torch.autograd.Function):
                 _ptr(f_grad), _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_forward_dynamics_backward")
         return table_grad, q_grad, qd_grad, f_grad, None, None, None
+
+
+class ForwardDynamicsRolloutFunction(torch.autograd.Function):
+    """(table, q0, qd0, f) -> (q, qd, qdd) of a forward-dynamics rollout; one rollout launch forward, the ABA adjoint
+    stepped in reverse time backward (drmb200_forward_dynamics_rollout_backward)."""
+
+    @staticmethod
+    def forward(ctx, table, q0, qd0, f, topo, flags, dt):
+        table, q0, qd0, f = table.contiguous(), q0.contiguous(), qd0.contiguous(), f.contiguous()
+        q, qd, qdd = forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags)
+        ctx.save_for_backward(table, q0, qd0, f, q, qd)
+        ctx.topo, ctx.flags, ctx.dt = topo, flags, dt
+        return q, qd, qdd
+
+    @staticmethod
+    def backward(ctx, g_q, g_qd, g_qdd):
+        table, q0, qd0, f, q, qd = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        T, B, n = f.shape
+        g = [None if t is None else t.contiguous() for t in (g_q, g_qd, g_qdd)]
+        _require_cuda(*g)
+        table_grad = torch.zeros_like(table) if need[0] else None
+        alloc = torch.zeros_like if T == 0 else torch.empty_like       # zero steps: the state passes through unchanged
+        q0_grad = alloc(q0) if need[1] else None
+        qd0_grad = alloc(q0) if need[2] else None
+        f_grad = torch.empty_like(f) if need[3] else None
+        nbytes = int(lib().drmb200_forward_dynamics_rollout_backward_workspace_bytes(ctypes.byref(ctx.topo), B))
+        ws = torch.empty((max(nbytes, 4) + 3) // 4, device=q0.device, dtype=torch.float32)
+        with _on(q0.device):
+            rc = lib().drmb200_forward_dynamics_rollout_backward(
+                ctypes.byref(ctx.topo), _ptr(table), _ptr(q0), _ptr(qd0), _ptr(f), B, T, ctypes.c_float(ctx.dt), ctx.flags,
+                _ptr(q), _ptr(qd), _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(q0_grad), _ptr(qd0_grad), _ptr(f_grad),
+                _ptr(table_grad), _ptr(ws), _stream())
+        _check(rc, "drmb200_forward_dynamics_rollout_backward")
+        return table_grad, q0_grad, qd0_grad, f_grad, None, None, None
 
 
 def mass_matrix_raw(topo, table, q, out=None, folded=None):

@@ -405,6 +405,51 @@ class DifferentiableRobotModel(torch.nn.Module):
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
         return engine.ForwardDynamicsFunction.apply(self._link_table(), q, qd, f, self._topology, flags, self._folded_table())
 
+    def compute_forward_dynamics_rollout(
+        self,
+        q0: torch.Tensor,
+        qd0: torch.Tensor,
+        f: torch.Tensor,
+        dt: float,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = False,
+    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        r"""Integrate :meth:`compute_forward_dynamics` over ``T`` steps of semi-implicit (symplectic) Euler in ONE launch
+        (``csrc/rollout.cu``).  From ``(q_0, qd_0) = (q0, qd0)``, step ``t`` computes in fp32, in this order::
+
+            qdd_t = compute_forward_dynamics(q_t, qd_t, f[t], include_gravity, use_damping)
+            qd_{t+1} = qd_t + dt * qdd_t
+            q_{t+1} = q_t + dt * qd_{t+1}
+
+        and the result is bit-identical to that Python loop on the same model.
+
+        Args:
+            q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
+            f: applied joint forces of every step [T x batch_size x n_dofs] (or [T x n_dofs]); never modified
+            dt: step length in seconds (not differentiable)
+        Returns: time-major ``(q, qd, qdd)``, each [T x batch_size x n_dofs] (or [T x n_dofs]), with ``q[t] = q_{t+1}``,
+        ``qd[t] = qd_{t+1}`` and ``qdd[t] = qdd_t``.  Differentiable w.r.t. q0, qd0, f and every learnable link parameter
+        (the articulated-body adjoint stepped backwards in time).  Argument errors raise ``AssertionError``."""
+        for name, t in (("q0", q0), ("qd0", qd0), ("f", f)):
+            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
+            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
+            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
+        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
+        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
+        assert q0.shape[-1] == self._n_dofs, f"expected {self._n_dofs} joints, got {q0.shape[-1]}"
+        assert f.ndim == q0.ndim + 1 and f.shape[1:] == q0.shape, "f must be [T x batch_size x n_dofs] (or [T x n_dofs])."
+        squeeze = q0.ndim == 1
+        if squeeze:
+            q0, qd0, f = q0.unsqueeze(0), qd0.unsqueeze(0), f.unsqueeze(1)
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table()
+        dt = float(dt)
+        if torch.is_grad_enabled() and (table.requires_grad or q0.requires_grad or qd0.requires_grad or f.requires_grad):
+            out = engine.ForwardDynamicsRolloutFunction.apply(table, q0, qd0, f, self._topology, flags, dt)
+        else:
+            out = engine.forward_dynamics_rollout_raw(self._topology, table, q0, qd0, f, dt, flags)
+        return tuple(o[:, 0] for o in out) if squeeze else tuple(out)
+
     @tensor_check
     def compute_forward_dynamics_crba(
         self,

@@ -18,6 +18,8 @@
  *   drmb200_inverse_dynamics_backward    analytic adjoint of RNEA (SURVEY.md Appendix B.2).
  *   drmb200_forward_dynamics   replaces  compute_forward_dynamics (robot_model.py:488-624), the articulated-body
  *                                        algorithm, in one launch.
+ *   drmb200_forward_dynamics_rollout     many semi-implicit Euler steps of the above in one launch (the reference
+ *                                        integrates with a Python loop around compute_forward_dynamics), and its adjoint.
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -235,6 +237,42 @@ int drmb200_forward_dynamics_backward(const drmb200_topology_t* topo,
                                       int64_t batch, uint32_t flags, const float* g_qdd,
                                       float* q_grad, float* qd_grad, float* f_grad,
                                       float* table_grad, void* workspace, void* cuda_stream);
+
+/*
+ * Forward-dynamics rollout: n_steps steps of semi-implicit (symplectic) Euler over drmb200_forward_dynamics in ONE launch.
+ * Starting from (q_0, qd_0) = (q0, qd0), step t = 0 .. n_steps-1 computes, in fp32 and in exactly this order,
+ *     qdd_t = FD(q_t, qd_t, f_t);   qd_{t+1} = qd_t + dt * qdd_t;   q_{t+1} = q_t + dt * qd_{t+1}
+ * (each "+ dt *" a rounded multiply, then a rounded add -- no FMA), so the trajectory is bit-identical to a loop of
+ * drmb200_forward_dynamics launches followed by those two updates.  flags mean what they mean for drmb200_forward_dynamics.
+ * Layout is time-major:
+ *   q0, qd0              [B, n_dofs]
+ *   f                    [n_steps, B, n_dofs]   applied joint forces of every step (never modified)
+ *   q, qd                [n_steps, B, n_dofs]   q[t] = q_{t+1}, qd[t] = qd_{t+1}
+ *   qdd                  [n_steps, B, n_dofs]   qdd[t] = qdd_t; may be NULL
+ * The table is staged (and folded) once per CTA and the state stays in shared memory for all steps.  Outputs must not alias
+ * inputs.  batch == 0 or n_steps == 0 is a no-op.
+ */
+int drmb200_forward_dynamics_rollout(const drmb200_topology_t* topo, const float* table,
+                                     const float* q0, const float* qd0, const float* f, int64_t batch, int32_t n_steps,
+                                     float dt, uint32_t flags, float* q, float* qd, float* qdd, void* cuda_stream);
+
+/*
+ * Adjoint of drmb200_forward_dynamics_rollout.  q / qd are the forward's outputs (the step inputs of steps 1 .. n_steps-1);
+ * g_q / g_qd / g_qdd [n_steps, B, n_dofs] are the upstream gradients of q / qd / qdd (NULL = zero).  Writes q0_grad /
+ * qd0_grad [B, n_dofs] and f_grad [n_steps, B, n_dofs] (each may be NULL) and accumulates the table gradient of all steps
+ * into table_grad (may be NULL).  Runs the analytic adjoint of drmb200_forward_dynamics_backward once per step, t = n_steps-1
+ * .. 0, with one element-wise launch per step between them (2 n_steps + 2 launches).  `workspace` must hold
+ * drmb200_forward_dynamics_rollout_backward_workspace_bytes(topo, batch) bytes; it does not depend on n_steps.  Outputs
+ * must not alias inputs.
+ */
+int64_t drmb200_forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch);
+int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, const float* table,
+                                              const float* q0, const float* qd0, const float* f, int64_t batch,
+                                              int32_t n_steps, float dt, uint32_t flags,
+                                              const float* q, const float* qd,
+                                              const float* g_q, const float* g_qd, const float* g_qdd,
+                                              float* q0_grad, float* qd0_grad, float* f_grad,
+                                              float* table_grad, void* workspace, void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state

@@ -5,6 +5,8 @@
   config 4  Allegro hand FK + Jacobian of one fingertip, per-GPU shard 32 768 and 2^21
   config 5  Kuka iiwa FK+Jacobian + RNEA forward, then backward with mass / com / inertia_mat of links 1..7
             learnable, per-GPU shard 131 072
+  rollout   Kuka iiwa forward-dynamics rollouts (BENCH_ONLY=rollout): the one-launch rollout kernel and its stepped
+            adjoint against the Python loop of compute_forward_dynamics, eager and CUDA-graphed
 
 CUDA-event timing on the launching stream, >= 5 warm-up iterations, inputs rotated over buffer sets
 larger than L2.  Prints one JSON object; copy it to profiles/ to have it judged.
@@ -174,6 +176,119 @@ def bench_forward_dynamics(stem_cls, batch):
         cr.forward_dynamics(nq, nqd, nf, True, True)
         res["cpu_c_port_configs_per_s"] = batch / (time.perf_counter() - t0)
         res["cpu_c_port_cores"] = os.cpu_count()
+    return res
+
+
+def gpu_identity():
+    """Name and power limit of the card, read in the same run as the numbers they qualify."""
+    import subprocess
+    try:
+        return subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as exc:
+        return f"nvidia-smi failed: {exc!r}"
+
+
+def _event_ms(fn, iters, warmup=3, graphed=False):
+    """ms per call of fn(); graphed: fn captured once in a CUDA graph (after warm-up on a side stream) and replayed."""
+    if graphed:
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(warmup):
+                fn()
+        torch.cuda.current_stream().wait_stream(side)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            fn()
+        run = g.replay
+    else:
+        run = fn
+    for _ in range(warmup):
+        run()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        run()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+def bench_rollout(batch, steps, iters=10):
+    """Kuka forward-dynamics rollout of `steps` semi-implicit Euler steps (gravity + damping, dt = 1 ms).
+    fused: drmb200_forward_dynamics_rollout (one launch) / its adjoint (2T + 2 launches, input and table gradients of
+    a learnable model); loop: compute_forward_dynamics + `qd = qd + dt * qdd; q = q + dt * qd` per step, through autograd
+    for the backward.  Both eager and replayed from a CUDA graph.
+    Algorithmic HBM bytes per configuration-step: forward 16n (f in; q, qd, qdd out), backward 28n (q_t, qd_t, f_t and the
+    three upstream gradients in, f_grad out)."""
+    m = drm.DifferentiableKUKAiiwa(device=DEV)
+    for i in range(1, 8):                                  # the system-identification setting: inertial parameters learnable
+        b = m._bodies[i]
+        m.make_link_param_learnable(b.name, "mass", UnconstrainedScalar(init_val=b.inertia.mass().detach().clone()))
+        m.make_link_param_learnable(b.name, "com", UnconstrainedTensor(1, 3, init_tensor=b.inertia.com().detach().clone()))
+        m.make_link_param_learnable(b.name, "inertia_mat", UnconstrainedTensor(
+            3, 3, init_tensor=b.inertia.inertia_mat().detach().clone().reshape(3, 3)))
+    m.fuse_learnable_parameters()
+    robot = O.load_robot(m.urdf_path, torch.float32)
+    n = robot.n_dofs
+    q0, qd0, _ = (t.to(DEV) for t in O.sample_inputs(robot, batch, seed=0, vel_scale=0.02))
+    f = 0.05 * torch.randn(steps, batch, n, device=DEV)
+    G = torch.randn(steps, batch, n, device=DEV)
+    dt = 1e-3
+
+    def loop(q, qd, ff):
+        qs, qds, qdds = [], [], []
+        for t in range(steps):
+            qdd = m.compute_forward_dynamics(q, qd, ff[t], True, True)
+            qd = qd + dt * qdd
+            q = q + dt * qd
+            qs.append(q)
+            qds.append(qd)
+            qdds.append(qdd)
+        return torch.stack(qs), torch.stack(qds), torch.stack(qdds)
+
+    def fused(q, qd, ff):
+        return m.compute_forward_dynamics_rollout(q, qd, ff, dt, True, True)
+
+    fa = f.clone().requires_grad_(True)
+
+    def fwd(impl):
+        def run():
+            with torch.no_grad():
+                impl(q0, qd0, f)
+        return run
+
+    def fwd_bwd(impl):
+        def run():
+            m.fused_link_params.flat.grad = None
+            fa.grad = None
+            q, qd, qdd = impl(q0, qd0, fa)
+            ((q + qd + qdd) * G).sum().backward()
+        return run
+
+    cs = batch * steps
+    res = {"batch": batch, "steps": steps, "dt": dt, "configuration_steps": cs,
+           "rollout_tile": 64 if (batch + 63) // 64 >= torch.cuda.get_device_properties(0).multi_processor_count else 32,
+           "algorithmic_bytes_per_configuration_step": {"forward": 16 * n, "backward": 28 * n}}
+    for name, fn in (("fused_forward", fwd(fused)), ("loop_forward", fwd(loop)),
+                     ("fused_forward_backward", fwd_bwd(fused)), ("loop_forward_backward", fwd_bwd(loop))):
+        for mode in ("eager", "graphed"):
+            try:
+                ms = _event_ms(fn, iters, graphed=(mode == "graphed"))
+            except Exception as exc:                                    # report, do not hide
+                res[f"{name}_{mode}_error"] = repr(exc)[:300]
+                continue
+            res[f"{name}_{mode}_ms"] = ms
+            res[f"{name}_{mode}_configuration_steps_per_s"] = cs / ms * 1e3
+    ms = res.get("fused_forward_eager_ms")
+    if ms:
+        res["fused_forward_achieved_GBps"] = cs * 16 * n / ms / 1e6
+    before = engine.launch_count()
+    fwd_bwd(fused)()
+    torch.cuda.synchronize()
+    res["fused_forward_backward_launches"] = engine.launch_count() - before
     return res
 
 
@@ -365,7 +480,12 @@ def bench_train_step(batch, fused=False):
 
 
 def main():
-    out = {"peak_GBps": PEAK, "gpu": torch.cuda.get_device_name(0)}
+    out = {"peak_GBps": PEAK, "gpu": torch.cuda.get_device_name(0), "gpu_name_power_limit_max_sm_clock": gpu_identity()}
+    if os.environ.get("BENCH_ONLY") == "rollout":
+        # 4096 configurations leave a 64-wide tile short of one CTA per SM (32-wide tiles are chosen); 65 536 fill them
+        out["kuka_rollout"] = [bench_rollout(4096, 256), bench_rollout(65536, 64)]
+        print(json.dumps(out))
+        return
     if os.environ.get("BENCH_ONLY") == "config5":
         out["config5_kuka_train_step"] = [bench_train_step(131072, fused=False), bench_train_step(131072, fused=True)]
         print(json.dumps(out))
@@ -408,6 +528,7 @@ def main():
     out["kuka_mass_matrix"] = [bench_mass_matrix(drm.DifferentiableKUKAiiwa, b) for b in (65536, 1 << 20)]
     out["kuka_kinematic_state"] = [bench_kinematic_state(drm.DifferentiableKUKAiiwa, 1 << 20)]
     out["kuka_forward_dynamics"] =[bench_forward_dynamics(drm.DifferentiableKUKAiiwa, b) for b in (65536, 1 << 20)]
+    out["kuka_rollout"] = [bench_rollout(4096, 256), bench_rollout(65536, 64)]
     print(json.dumps(out))
 
 
