@@ -49,6 +49,16 @@ def cuda(a, grad=False):
     return t.requires_grad_(True) if grad else t
 
 
+def shifted(x):
+    """The same values in a fresh contiguous tensor whose base address is 4 bytes past a 16-byte boundary: kernels must take
+    their cooperative-copy staging instead of TMA bulk copies / float4 accesses for it."""
+    buf = x.new_empty(x.numel() + 1)
+    buf[1:].copy_(x.reshape(-1))
+    out = buf[1:].view_as(x)
+    assert out.data_ptr() % 16 != 0 and out.is_contiguous()
+    return out
+
+
 def check_against_golden(g, prefix, params, input_grads):
     scale = max(float(np.abs(g[k]).max()) for k in g.files if k.startswith(prefix + "."))
     tol = dict(rtol=2e-4, atol=2e-5 * max(scale, 1.0))
@@ -325,11 +335,6 @@ def test_chain_adjoint_kernel_matches_the_tree_kernel(stem, batch):
     G = torch.randn(batch, n, device=DEV)
     learn, params = learnable_model(stem)
     const = drm.DifferentiableRobotModel(urdf_path(stem), stem, device=DEV)
-
-    def shifted(x):                      # the same values at an address that is not a multiple of 16 bytes
-        buf = torch.empty(x.numel() + 1, device=DEV)
-        buf[1:].copy_(x.reshape(-1))
-        return buf[1:].view_as(x)
 
     def run(model, unaligned, grav, damp):
         for p in params.values():

@@ -74,15 +74,24 @@ def test_fk_jacobian_matches_reference_golden(robot_stem, fk_variant):
     assert engine.launch_count() - launches == 3 * len(g["fk_links"])
 
 
-@pytest.fixture(params=[(1, 1), (0, 1), (1, 0), (0, 0)], ids=["packed_folded", "scalar_folded", "packed_every_link", "scalar_every_link"])
+@pytest.fixture(params=[(1, 1, 0), (0, 1, 0), (1, 0, 0), (0, 0, 0), (1, 1, 64), (1, 1, 128), (0, 0, 128)],
+                ids=["packed_folded", "scalar_folded", "packed_every_link", "scalar_every_link", "packed_folded_tile64",
+                     "packed_folded_tile128", "scalar_every_link_tile128"])
 def rnea_variant(request):
     """Both arithmetic variants of the inverse-dynamics kernel, with fixed links folded into their movable ancestors
-    (default) and with one step per link like the reference, must give the same parity."""
-    engine.set_option("rnea_packed", request.param[0])
-    engine.set_option("rnea_fold", request.param[1])
-    yield request.param
-    engine.set_option("rnea_packed", 1)
-    engine.set_option("rnea_fold", 1)
+    (default) and with one step per link like the reference, must give the same parity.  The tile ("rnea_tile") is
+    picked by batch size (64 rows below 32 768 configurations); forcing 128 runs the small and ragged batches here with
+    the large-batch tile."""
+    packed, fold, tile = request.param
+    try:
+        engine.set_option("rnea_packed", packed)
+        engine.set_option("rnea_fold", fold)
+        engine.set_option("rnea_tile", tile)
+        yield request.param
+    finally:
+        engine.set_option("rnea_packed", 1)
+        engine.set_option("rnea_fold", 1)
+        engine.set_option("rnea_tile", 0)
 
 
 def test_inverse_dynamics_matches_reference_golden(robot_stem, rnea_variant):
