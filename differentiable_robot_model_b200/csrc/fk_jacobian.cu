@@ -462,8 +462,13 @@ template <int NDOF, int TILE, bool WITH_JAC, int MAXLEN>
 static int launch_fk(const PathProgram& prog, const FkArgs& args, cudaStream_t stream) {
     const FkSmemLayout L(TILE, prog.n_dofs, prog.len, WITH_JAC);
     const size_t smem_bytes = (size_t)L.total_floats * sizeof(float);
-    if (smem_bytes > 227 * 1024) { set_error("fk kernel needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
     auto kern = fk_jacobian_kernel<NDOF, TILE, WITH_JAC, MAXLEN>;
+    cudaFuncAttributes fa;
+    const size_t static_bytes = cudaFuncGetAttributes(&fa, kern) == cudaSuccess ? fa.sharedSizeBytes : 1024;
+    if (smem_bytes + static_bytes > 227 * 1024) {
+        set_error("fk kernel needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes + static_bytes);
+        return DRMB200_ELIMIT;
+    }
     static size_t configured_by_dev[64] = {0};     // per instantiation, per device
     int dev = 0;
     cudaGetDevice(&dev);
@@ -638,6 +643,10 @@ int fk_jacobian_device(const drmb200_topology_t* topo, int32_t ee_link, const fl
     int tile = get_option(1);
     if (tile != 64 && tile != 128 && tile != 256)
         tile = (prog.n_dofs > 8 || (batch <= (int64_t)device_sm_count() * 1024 && args.pdl != 2)) ? 128 : 64;
+    // a long path with many Jacobian columns (e.g. a 63-DoF chain) does not fit 128 rows: take 64 (the kernel's static
+    // shared memory counts against the same 227 KB, hence the margin)
+    if (tile == 128 && (size_t)FkSmemLayout(128, prog.n_dofs, prog.len, with_jac).total_floats * sizeof(float) + 1024 > 227 * 1024)
+        tile = 64;
     switch (prog.n_dofs) {
         case 2: return launch_fk_t<2>(tile, with_jac, prog, args, stream);
         case 7: return launch_fk_t<7>(tile, with_jac, prog, args, stream);

@@ -20,6 +20,7 @@ Reference lines followed (relative to /root/reference/differentiable_robot_model
   forward_kinematics      robot_model.py:224-248
   jacobian                robot_model.py:627-667
   inverse_dynamics        robot_model.py:251-375, spatial_vector_algebra.py:204-224, 281-291, 321-338
+  dynamic_state           robot_model.py:183-193, 262-301 (the per-link state inverse_dynamics computes)
 """
 import os
 import sys
@@ -268,6 +269,19 @@ def _inertia_times(robot, i, ang, lin):
 
 def inverse_dynamics(robot, q, qd, qdd, include_gravity=True, use_damping=True):
     """RNEA (robot_model.py:251-375)."""
+    return _rnea(robot, q, qd, qdd, include_gravity, use_damping)["tau"]
+
+
+def dynamic_state(robot, q, qd, qdd, include_gravity=True, use_damping=True):
+    """The per-link state the reference leaves in its bodies after compute_inverse_dynamics (robot_model.py:183-193,
+    262-301), from the same evaluation as inverse_dynamics: dict of [N, B, 3] tensors "vel_ang", "vel_lin" (body-frame
+    spatial velocity), "acc_ang", "acc_lin" (al, a: spatial acceleration, gravity as a base acceleration),
+    "force_ang", "force_lin" (body wrench with the wrenches of all descendants accumulated), plus "tau" [B, n]."""
+    s = _rnea(robot, q, qd, qdd, include_gravity, use_damping)
+    return {k: (v if k == "tau" else torch.stack(v)) for k, v in s.items()}
+
+
+def _rnea(robot, q, qd, qdd, include_gravity, use_damping):
     B = q.shape[0]
     N = len(robot.names)
     R, p, w, v, joints = kinematic_state(robot, q, qd)
@@ -311,10 +325,10 @@ def inverse_dynamics(robot, q, qd, qdd, include_gravity=True, use_damping=True):
         ax = robot.axis[i]
         k = int(torch.where(ax != 0)[0])                          # robot_model.py:357
         cols.append(torch.sign(ax[k]) * f_ang[i][:, k])
-    tau = torch.stack(cols, dim=1)
-    if use_damping:
+    tau = torch.stack(cols, dim=1) if cols else q.new_zeros(B, 0)
+    if use_damping and cols:
         tau = tau + torch.stack([robot.damping[i] for i in robot.controlled]).unsqueeze(0) * qd
-    return tau
+    return {"tau": tau, "vel_ang": w, "vel_lin": v, "acc_ang": al, "acc_lin": a, "force_ang": f_ang, "force_lin": f_lin}
 
 
 def _spatial_inertia(robot, i):
