@@ -102,6 +102,10 @@ int64_t forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology
 int forward_dynamics_rollout_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*,
                                              int64_t, int32_t, float, uint32_t, const float*, const float*, const float*,
                                              const float*, const float*, float*, float*, float*, float*, void*, cudaStream_t);
+int inverse_dynamics_derivatives_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
+                                        uint32_t, float*, float*, cudaStream_t, bool);
+int forward_dynamics_derivatives_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
+                                        uint32_t, float*, float*, float*, cudaStream_t, bool);
 int64_t table_grad_workspace_bytes(const drmb200_topology_t*, int64_t);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 int mass_matrix_device(const drmb200_topology_t*, const float*, const float*, int64_t, float*, cudaStream_t);
@@ -375,6 +379,34 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
     return drm::forward_dynamics_rollout_backward_device(topo, table, q0, qd0, f, batch, n_steps, dt, flags, q, qd, g_q, g_qd,
                                                          g_qdd, q0_grad, qd0_grad, f_grad, table_grad, workspace,
                                                          static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_inverse_dynamics_derivatives(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
+                                         const float* qdd, int64_t batch, uint32_t flags, float* dtau_dq, float* dtau_dqd,
+                                         void* cuda_stream) {
+    return drm::inverse_dynamics_derivatives_device(topo, table, q, qd, qdd, batch, flags, dtau_dq, dtau_dqd,
+                                                    static_cast<cudaStream_t>(cuda_stream), false);
+}
+
+int drmb200_inverse_dynamics_derivatives_prefolded(const drmb200_topology_t* topo, const float* folded, const float* q,
+                                                   const float* qd, const float* qdd, int64_t batch, uint32_t flags,
+                                                   float* dtau_dq, float* dtau_dqd, void* cuda_stream) {
+    return drm::inverse_dynamics_derivatives_device(topo, folded, q, qd, qdd, batch, flags, dtau_dq, dtau_dqd,
+                                                    static_cast<cudaStream_t>(cuda_stream), true);
+}
+
+int drmb200_forward_dynamics_derivatives(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
+                                         const float* f, int64_t batch, uint32_t flags, float* dqdd_dq, float* dqdd_dqd,
+                                         float* dqdd_df, void* cuda_stream) {
+    return drm::forward_dynamics_derivatives_device(topo, table, q, qd, f, batch, flags, dqdd_dq, dqdd_dqd, dqdd_df,
+                                                    static_cast<cudaStream_t>(cuda_stream), false);
+}
+
+int drmb200_forward_dynamics_derivatives_prefolded(const drmb200_topology_t* topo, const float* folded, const float* q,
+                                                   const float* qd, const float* f, int64_t batch, uint32_t flags,
+                                                   float* dqdd_dq, float* dqdd_dqd, float* dqdd_df, void* cuda_stream) {
+    return drm::forward_dynamics_derivatives_device(topo, folded, q, qd, f, batch, flags, dqdd_dq, dqdd_dqd, dqdd_df,
+                                                    static_cast<cudaStream_t>(cuda_stream), true);
 }
 
 int drmb200_kinematic_state(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -78,6 +78,18 @@ _SIGNATURES = {
                                                                  ctypes.c_uint32, _c_float_p, _c_float_p, _c_float_p,
                                                                  _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                                  _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_inverse_dynamics_derivatives": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
+                                                            _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p, _c_float_p,
+                                                            ctypes.c_void_p]),
+    "drmb200_inverse_dynamics_derivatives_prefolded": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
+                                                                      _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p,
+                                                                      _c_float_p, ctypes.c_void_p]),
+    "drmb200_forward_dynamics_derivatives": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
+                                                            _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p, _c_float_p,
+                                                            _c_float_p, ctypes.c_void_p]),
+    "drmb200_forward_dynamics_derivatives_prefolded": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
+                                                                      _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p,
+                                                                      _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_kinematic_state": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
                                                _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table": (ctypes.c_int, [_c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_void_p]),
@@ -283,6 +295,44 @@ def forward_dynamics_raw(topo, table, q, qd, f, flags, out=None, folded=None):
                                                 flags, _ptr(qdd), _stream())
     _check(rc, "drmb200_forward_dynamics")
     return qdd
+
+
+def inverse_dynamics_derivatives_raw(topo, table, q, qd, qdd, flags, folded=None, want_dq=True, want_dqd=True):
+    """(dtau_dq, dtau_dqd) [B, n, n], out[b, i, j] = d tau_i / d x_j, one launch (drmb200_inverse_dynamics_derivatives;
+    `folded`: rows of fold_link_table for an unchanged table).  A matrix that is not wanted is None."""
+    _require_cuda(table, q, qd, qdd, folded)
+    q, qd, qdd = q.contiguous(), qd.contiguous(), qdd.contiguous()
+    B, n = q.shape
+    dq = torch.empty((B, n, n), device=q.device, dtype=torch.float32) if want_dq else None
+    dqd = torch.empty((B, n, n), device=q.device, dtype=torch.float32) if want_dqd else None
+    with _on(q.device):
+        if folded is not None:
+            rc = lib().drmb200_inverse_dynamics_derivatives_prefolded(ctypes.byref(topo), _ptr(folded), _ptr(q), _ptr(qd), _ptr(qdd),
+                                                                      B, flags & 3, _ptr(dq), _ptr(dqd), _stream())
+        else:
+            rc = lib().drmb200_inverse_dynamics_derivatives(ctypes.byref(topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(qdd), B,
+                                                            flags & 3, _ptr(dq), _ptr(dqd), _stream())
+    _check(rc, "drmb200_inverse_dynamics_derivatives")
+    return dq, dqd
+
+
+def forward_dynamics_derivatives_raw(topo, table, q, qd, f, flags, folded=None, want_dq=True, want_dqd=True, want_df=True):
+    """(dqdd_dq, dqdd_dqd, dqdd_df) [B, n, n], out[b, i, j] = d qdd_i / d x_j, one launch
+    (drmb200_forward_dynamics_derivatives; `folded`: rows of fold_link_table for an unchanged table)."""
+    _require_cuda(table, q, qd, f, folded)
+    q, qd, f = q.contiguous(), qd.contiguous(), f.contiguous()
+    B, n = q.shape
+    outs = [torch.empty((B, n, n), device=q.device, dtype=torch.float32) if want else None
+            for want in (want_dq, want_dqd, want_df)]
+    with _on(q.device):
+        if folded is not None:
+            rc = lib().drmb200_forward_dynamics_derivatives_prefolded(ctypes.byref(topo), _ptr(folded), _ptr(q), _ptr(qd), _ptr(f),
+                                                                      B, flags & 3, *[_ptr(o) for o in outs], _stream())
+        else:
+            rc = lib().drmb200_forward_dynamics_derivatives(ctypes.byref(topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B,
+                                                            flags & 3, *[_ptr(o) for o in outs], _stream())
+    _check(rc, "drmb200_forward_dynamics_derivatives")
+    return tuple(outs)
 
 
 def forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags, want_qdd=True):

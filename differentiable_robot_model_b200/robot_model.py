@@ -405,6 +405,55 @@ class DifferentiableRobotModel(torch.nn.Module):
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
         return engine.ForwardDynamicsFunction.apply(self._link_table(), q, qd, f, self._topology, flags, self._folded_table())
 
+    @tensor_check
+    def compute_inverse_dynamics_derivatives(
+        self,
+        q: torch.Tensor,
+        qd: torch.Tensor,
+        qdd_des: torch.Tensor,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = True,
+    ) -> Tuple[torch.Tensor, torch.Tensor]:
+        r"""Jacobians of :meth:`compute_inverse_dynamics` in ONE launch (``csrc/dynamics_derivatives.cu``, forward-mode RNEA).
+
+        Args:
+            q, qd, qdd_des: joint angles / velocities / desired accelerations [batch_size x n_dofs]
+            include_gravity, use_damping: as for :meth:`compute_inverse_dynamics`
+        Returns: ``(dtau_dq, dtau_dqd)``, each [batch_size x n_dofs x n_dofs] (``[n_dofs x n_dofs]`` for 1-D inputs) with
+        ``out[b, i, j] = d tau_i / d x_j``.  The outputs carry no autograd graph: they use the current values of the link
+        parameters (learnable and fused ones included) but are not differentiable themselves."""
+        self._check_q(q, qd, qdd_des)
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table().detach()
+        return engine.inverse_dynamics_derivatives_raw(self._topology, table, q.detach(), qd.detach(), qdd_des.detach(), flags,
+                                                       folded=self._folded_table())
+
+    @tensor_check
+    def compute_forward_dynamics_derivatives(
+        self,
+        q: torch.Tensor,
+        qd: torch.Tensor,
+        f: torch.Tensor,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = False,
+    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        r"""Jacobians of :meth:`compute_forward_dynamics` in ONE launch (``csrc/dynamics_derivatives.cu``, forward-mode
+        articulated-body algorithm).
+
+        Args:
+            q, qd, f: joint angles / velocities / applied joint forces [batch_size x n_dofs]
+            include_gravity, use_damping: as for :meth:`compute_forward_dynamics`
+        Returns: ``(dqdd_dq, dqdd_dqd, dqdd_df)``, each [batch_size x n_dofs x n_dofs] (``[n_dofs x n_dofs]`` for 1-D
+        inputs) with ``out[b, i, j] = d qdd_i / d x_j``.  They differentiate the articulated-body arithmetic itself, so they
+        are exact for non-symmetric ``inertia_mat`` too, where ``-H^-1 dtau`` is not.  The outputs carry no autograd graph:
+        they use the current values of the link parameters (learnable and fused ones included) but are not differentiable
+        themselves."""
+        self._check_q(q, qd, f)
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table().detach()
+        return engine.forward_dynamics_derivatives_raw(self._topology, table, q.detach(), qd.detach(), f.detach(), flags,
+                                                       folded=self._folded_table())
+
     def compute_forward_dynamics_rollout(
         self,
         q0: torch.Tensor,

@@ -20,6 +20,8 @@
  *                                        algorithm, in one launch.
  *   drmb200_forward_dynamics_rollout     many semi-implicit Euler steps of the above in one launch (the reference
  *                                        integrates with a Python loop around compute_forward_dynamics), and its adjoint.
+ *   drmb200_inverse_dynamics_derivatives / drmb200_forward_dynamics_derivatives   the Jacobians of the two above w.r.t.
+ *                                        q, qd (and f), [B, n, n] each, one launch (the reference: autograd, row by row).
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -273,6 +275,35 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
                                               const float* g_q, const float* g_qd, const float* g_qdd,
                                               float* q0_grad, float* qd0_grad, float* f_grad,
                                               float* table_grad, void* workspace, void* cuda_stream);
+
+/*
+ * Jacobians of the dynamics, one launch each (forward-mode recursions, csrc/dynamics_derivatives.cu).  Every matrix is
+ * [B, n_dofs, n_dofs], row-major per configuration, out[b, i, j] = d y_i / d x_j of exactly what drmb200_inverse_dynamics /
+ * drmb200_forward_dynamics compute with the same flags and table (any inertia matrix, non-symmetric ones included: the
+ * forward-dynamics derivatives differentiate the articulated-body arithmetic itself, not -H^-1 dtau).
+ *   drmb200_inverse_dynamics_derivatives   dtau_dq, dtau_dqd
+ *   drmb200_forward_dynamics_derivatives   dqdd_dq, dqdd_dqd, dqdd_df   (dqdd_df[:, :, j] = forward dynamics at (q, 0, e_j)
+ *                                          without gravity or damping: the articulated-body algorithm is affine in f)
+ * Caller-allocated outputs; NULL skips a matrix (all NULL: nothing is launched).  No allocation, no synchronisation: a call
+ * can be captured in a CUDA graph.  The *_prefolded variants read the rows of drmb200_fold_link_table.  A model whose
+ * per-CTA footprint exceeds 227 KB of shared memory even at one configuration per CTA returns DRMB200_ELIMIT (about 50 DoF
+ * for inverse dynamics and 38 for forward dynamics on a serial chain).
+ */
+int drmb200_inverse_dynamics_derivatives(const drmb200_topology_t* topo,
+                                         const float* table, const float* q, const float* qd, const float* qdd,
+                                         int64_t batch, uint32_t flags, float* dtau_dq, float* dtau_dqd, void* cuda_stream);
+int drmb200_inverse_dynamics_derivatives_prefolded(const drmb200_topology_t* topo,
+                                                   const float* folded, const float* q, const float* qd, const float* qdd,
+                                                   int64_t batch, uint32_t flags, float* dtau_dq, float* dtau_dqd,
+                                                   void* cuda_stream);
+int drmb200_forward_dynamics_derivatives(const drmb200_topology_t* topo,
+                                         const float* table, const float* q, const float* qd, const float* f,
+                                         int64_t batch, uint32_t flags, float* dqdd_dq, float* dqdd_dqd, float* dqdd_df,
+                                         void* cuda_stream);
+int drmb200_forward_dynamics_derivatives_prefolded(const drmb200_topology_t* topo,
+                                                   const float* folded, const float* q, const float* qd, const float* f,
+                                                   int64_t batch, uint32_t flags, float* dqdd_dq, float* dqdd_dqd,
+                                                   float* dqdd_df, void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state
