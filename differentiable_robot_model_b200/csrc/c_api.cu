@@ -106,6 +106,9 @@ int inverse_dynamics_derivatives_device(const drmb200_topology_t*, const float*,
                                         uint32_t, float*, float*, cudaStream_t, bool);
 int forward_dynamics_derivatives_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
                                         uint32_t, float*, float*, float*, cudaStream_t, bool);
+int inverse_kinematics_device(const drmb200_topology_t*, int32_t, const float*, const float*, const float*, const float*,
+                              const float*, const float*, const float*, int64_t, int32_t, float, float, float, float*, float*,
+                              float*, uint8_t*, float*, cudaStream_t);
 int64_t table_grad_workspace_bytes(const drmb200_topology_t*, int64_t);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 int mass_matrix_device(const drmb200_topology_t*, const float*, const float*, int64_t, float*, cudaStream_t);
@@ -407,6 +410,16 @@ int drmb200_forward_dynamics_derivatives_prefolded(const drmb200_topology_t* top
                                                    float* dqdd_dq, float* dqdd_dqd, float* dqdd_df, void* cuda_stream) {
     return drm::forward_dynamics_derivatives_device(topo, folded, q, qd, f, batch, flags, dqdd_dq, dqdd_dqd, dqdd_df,
                                                     static_cast<cudaStream_t>(cuda_stream), true);
+}
+
+int drmb200_inverse_kinematics(const drmb200_topology_t* topo, int32_t ee_link, const float* table, const float* q0,
+                               const float* target_pos, const float* target_quat, const float* lower, const float* upper,
+                               const float* damping_in, int64_t batch, int32_t max_iters, float damping_init, float pos_tol,
+                               float rot_tol, float* q, float* pos_err, float* rot_err, uint8_t* converged, float* damping_out,
+                               void* cuda_stream) {
+    return drm::inverse_kinematics_device(topo, ee_link, table, q0, target_pos, target_quat, lower, upper, damping_in, batch,
+                                          max_iters, damping_init, pos_tol, rot_tol, q, pos_err, rot_err, converged, damping_out,
+                                          static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_kinematic_state(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

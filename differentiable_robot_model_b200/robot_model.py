@@ -25,7 +25,7 @@ Deliberate deviations from the reference (see DESIGN.md):
 import contextlib
 import os
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
 import torch
 
@@ -78,6 +78,17 @@ def tensor_check(function):
     wrapper.__name__ = function.__name__
     wrapper.__doc__ = function.__doc__
     return wrapper
+
+
+class InverseKinematicsResult(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_inverse_kinematics` returns, per row: the joint angles, the position
+    and orientation errors at them (metres / radians; orientation 0 for position-only solves), whether both are within
+    tolerance, and the final Levenberg-Marquardt damping (pass it back as ``damping`` to continue a solve)."""
+    q: torch.Tensor
+    pos_error: torch.Tensor
+    rot_error: torch.Tensor
+    converged: torch.Tensor
+    damping: torch.Tensor
 
 
 class DifferentiableRobotModel(torch.nn.Module):
@@ -453,6 +464,68 @@ class DifferentiableRobotModel(torch.nn.Module):
         table = self._link_table().detach()
         return engine.forward_dynamics_derivatives_raw(self._topology, table, q.detach(), qd.detach(), f.detach(), flags,
                                                        folded=self._folded_table())
+
+    def compute_inverse_kinematics(
+        self,
+        q0: torch.Tensor,
+        link_name: str,
+        target_pos: torch.Tensor,
+        target_quat: Optional[torch.Tensor] = None,
+        max_iters: int = 100,
+        pos_tol: float = 1e-4,
+        rot_tol: float = 1e-3,
+        respect_joint_limits: bool = True,
+        damping: Optional[Union[float, torch.Tensor]] = None,
+    ) -> InverseKinematicsResult:
+        r"""Inverse kinematics of ``link_name``: up to ``max_iters`` damped least-squares (Levenberg-Marquardt) iterations
+        per row, all in ONE launch (``csrc/inverse_kinematics.cu``; the algorithm is stated in ``include/drm_b200.h``).
+
+        Args:
+            q0: start joint angles [batch_size x n_dofs] (clamped to the joint limits first)
+            link_name: the link whose frame should reach the target
+            target_pos: target position [batch_size x 3]
+            target_quat: target orientation [batch_size x 4], xyzw like :meth:`compute_forward_kinematics` (normalised
+                here); None solves for the position only
+            pos_tol, rot_tol: a row stops once its position error (m) and orientation error (rad) are both within these
+            respect_joint_limits: clamp every iterate to :meth:`get_joint_limits`
+            damping: initial damping, a float or one value per row [batch_size]; None: 1e-2
+        Returns: :class:`InverseKinematicsResult` ``(q, pos_error, rot_error, converged, damping)``, squeezed for 1-D
+        inputs.  Joints off the root -> link path are returned unchanged.  The outputs carry no autograd graph: they use the
+        current values of the link parameters (learnable and fused ones included) but are not differentiable."""
+        link_idx = self._name_to_idx_map[link_name]          # KeyError for unknown links
+        damping_init = engine.IK_DAMPING_INIT
+        per_row = None
+        if isinstance(damping, torch.Tensor):
+            per_row = damping.detach().unsqueeze(-1)          # [B, 1] (or [1] for 1-D inputs): batch-checked below
+        elif damping is not None:
+            damping_init = float(damping)
+        out = self._inverse_kinematics(q0, target_pos, target_quat, per_row, link_idx=link_idx, max_iters=int(max_iters),
+                                       damping_init=damping_init, pos_tol=float(pos_tol), rot_tol=float(rot_tol),
+                                       respect_joint_limits=respect_joint_limits)
+        return InverseKinematicsResult(*out)
+
+    @tensor_check
+    def _inverse_kinematics(self, q0, target_pos, target_quat, damping, link_idx, max_iters, damping_init, pos_tol, rot_tol,
+                            respect_joint_limits):
+        self._check_q(q0)
+        assert target_pos.shape[1] == 3, "target_pos must be [batch_size x 3]"
+        assert target_quat is None or target_quat.shape[1] == 4, "target_quat must be [batch_size x 4]"
+        lower, upper = self._joint_limit_tensors() if respect_joint_limits else (None, None)
+        table = self._link_table().detach()
+        q, pos_err, rot_err, converged, damp = engine.inverse_kinematics_raw(
+            self._topology, link_idx, table, q0.detach(), target_pos.detach(),
+            None if target_quat is None else target_quat.detach(), lower, upper,
+            None if damping is None else damping[:, 0], max_iters, damping_init, pos_tol, rot_tol)
+        return q, pos_err, rot_err, converged, damp
+
+    def _joint_limit_tensors(self):
+        """(lower, upper) [n_dofs] fp32 on the model's device, from get_joint_limits(), built once."""
+        if getattr(self, "_limit_cache", None) is None:
+            limits = self.get_joint_limits()
+            lower = torch.tensor([float(l["lower"]) for l in limits], dtype=torch.float32, device=self._device)
+            upper = torch.tensor([float(l["upper"]) for l in limits], dtype=torch.float32, device=self._device)
+            self._limit_cache = (lower, upper)
+        return self._limit_cache
 
     def compute_forward_dynamics_rollout(
         self,

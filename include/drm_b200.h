@@ -22,6 +22,8 @@
  *                                        integrates with a Python loop around compute_forward_dynamics), and its adjoint.
  *   drmb200_inverse_dynamics_derivatives / drmb200_forward_dynamics_derivatives   the Jacobians of the two above w.r.t.
  *                                        q, qd (and f), [B, n, n] each, one launch (the reference: autograd, row by row).
+ *   drmb200_inverse_kinematics           Levenberg-Marquardt inverse kinematics of one link for a batch of pose targets,
+ *                                        all iterations in one launch (the reference has no IK).
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -304,6 +306,35 @@ int drmb200_forward_dynamics_derivatives_prefolded(const drmb200_topology_t* top
                                                    const float* folded, const float* q, const float* qd, const float* f,
                                                    int64_t batch, uint32_t flags, float* dqdd_dq, float* dqdd_dqd,
                                                    float* dqdd_df, void* cuda_stream);
+
+/*
+ * Inverse kinematics of link `ee_link`: damped least-squares (Levenberg-Marquardt) iterations for a batch of targets in ONE
+ * launch, one thread per row, all iterations on chip (csrc/inverse_kinematics.cu).  Per row b, in fp32:
+ *   q <- clamp(q0[b], lower, upper) (fminf(fmaxf(x, lower), upper) per joint; skipped when both are NULL),
+ *   lambda <- damping_in[b] (damping_init when damping_in is NULL), then evaluate at q: the pose (p, R) and the geometric
+ *   Jacobian J [6, n] (as drmb200_fk_jacobian, J_lin over J_ang) and the error
+ *     e_pos = target_pos[b] - p;  q_err = quat* (x) conj(quat(R)) (quat* = target_quat[b] normalised, xyzw, quat(R) as
+ *     drmb200_fk_jacobian returns it), negated if its w < 0;  e_rot = 2 atan2(s, w) / s q_err.xyz, s = |q_err.xyz| (0 if
+ *     s == 0): the world-frame rotation vector of R* R^T.  target_quat == NULL: position only, e and J are the 3
+ *     position rows.  E = |e|^2; done = |e_pos| <= pos_tol && |e_rot| <= rot_tol.
+ *   max_iters times, skipping rows that are done: Cholesky of A = J J^T + lambda I (a pivot <= 0 or not finite rejects the
+ *   step); q' = clamp(q + J^T A^-1 e), evaluated as above; accept iff E' < E (then q, J, e, E <- the trial's and
+ *   lambda <- max(lambda / 2, 1e-5)), else lambda <- min(4 lambda, 1e5).
+ * Outputs at the returned q: q [B, n_dofs], pos_err / rot_err [B] (|e_pos|, |e_rot|; rot_err = 0 for position only),
+ * converged [B] (0 / 1: done) and damping_out [B] (the final lambda).  K iterations in one call are bit-identical to K
+ * calls with max_iters = 1 that pass q and damping_out on.  Joints off the root -> ee path never move.  The suggested
+ * damping_init is 1e-2.  Inputs: q0 [B, n_dofs], target_pos [B, 3], target_quat [B, 4] or NULL, lower / upper [n_dofs]
+ * (both or neither), damping_in [B] or NULL.  Device pointers, caller-allocated outputs that must not alias inputs; no
+ * allocation, no synchronisation (graph-capturable).  batch == 0 is a no-op.  DRMB200_EINVAL for a model without movable
+ * joints, an ee path without movable joints, max_iters < 0, negative tolerances, one limit pointer without the other or
+ * damping_init <= 0; DRMB200_ELIMIT when a 32-row CTA needs more than 227 KB of shared memory (14 n + 7 floats per row).
+ */
+int drmb200_inverse_kinematics(const drmb200_topology_t* topo, int32_t ee_link, const float* table,
+                               const float* q0, const float* target_pos, const float* target_quat,
+                               const float* lower, const float* upper, const float* damping_in,
+                               int64_t batch, int32_t max_iters, float damping_init, float pos_tol, float rot_tol,
+                               float* q, float* pos_err, float* rot_err, uint8_t* converged, float* damping_out,
+                               void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state
