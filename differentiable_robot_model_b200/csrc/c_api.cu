@@ -109,6 +109,9 @@ int forward_dynamics_derivatives_device(const drmb200_topology_t*, const float*,
 int inverse_kinematics_device(const drmb200_topology_t*, int32_t, const float*, const float*, const float*, const float*,
                               const float*, const float*, const float*, int64_t, int32_t, float, float, float, float*, float*,
                               float*, uint8_t*, float*, cudaStream_t);
+int inverse_kinematics_multi_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                                    const float*, const float*, const float*, const float*, int64_t, int32_t, float, float, float,
+                                    float*, float*, float*, uint8_t*, float*, cudaStream_t);
 int64_t table_grad_workspace_bytes(const drmb200_topology_t*, int64_t);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 int mass_matrix_device(const drmb200_topology_t*, const float*, const float*, int64_t, float*, cudaStream_t);
@@ -420,6 +423,16 @@ int drmb200_inverse_kinematics(const drmb200_topology_t* topo, int32_t ee_link, 
     return drm::inverse_kinematics_device(topo, ee_link, table, q0, target_pos, target_quat, lower, upper, damping_in, batch,
                                           max_iters, damping_init, pos_tol, rot_tol, q, pos_err, rot_err, converged, damping_out,
                                           static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_inverse_kinematics_multi(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                     const float* q0, const float* target_pos, const float* target_quat, const float* lower,
+                                     const float* upper, const float* damping_in, int64_t batch, int32_t max_iters,
+                                     float damping_init, float pos_tol, float rot_tol, float* q, float* pos_err, float* rot_err,
+                                     uint8_t* converged, float* damping_out, void* cuda_stream) {
+    return drm::inverse_kinematics_multi_device(topo, n_ee, ee_links, table, q0, target_pos, target_quat, lower, upper, damping_in,
+                                                batch, max_iters, damping_init, pos_tol, rot_tol, q, pos_err, rot_err, converged,
+                                                damping_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_kinematic_state(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -24,31 +24,11 @@
 // Outputs are [n_ee, B, ...] blocks.  Algorithmic HBM bytes per configuration: 4n + n_ee (28 + 24n)  (Allegro, 4 tips:
 // 64 + 4 * 412 = 1712 B, SURVEY.md section 8d).
 #include <cstring>
-#include "drm_common.cuh"
+#include "multi_program.cuh"
 
 namespace drm {
 
-constexpr int MT_MAX_EE = 8;
 constexpr int MT_WARPS_MAX = 4;
-
-struct MultiProgram {
-    int32_t n_steps;                       // links walked: union of the root -> ee paths, depth first, root excluded
-    int32_t n_dofs;
-    int32_t n_ee;
-    int32_t n_state_slots;                 // branch points whose (R, p) is spilled
-    int32_t n_jslots;                      // max number of movable links on any root -> ee path
-    int32_t n_root_ee;                     // requested links that ARE the root (identity pose, zero Jacobian)
-    int8_t link[DRMB200_MAX_LINKS];        // table row of step k
-    int8_t psrc[DRMB200_MAX_LINKS];        // parent state: -1 root (identity), 0 registers (previous step), 1 + s slot s
-    int8_t save[DRMB200_MAX_LINKS];        // -1, or the slot the state after this step is saved to
-    int8_t dof[DRMB200_MAX_LINKS];         // q / Jacobian column, -1 for fixed joints
-    int8_t jslot[DRMB200_MAX_LINKS];       // joint scratch slot (depth among the movable links of the path), or -1
-    int8_t ee[DRMB200_MAX_LINKS];          // -1, or the index (0 .. n_ee) of the end effector emitted after this step
-    int8_t axis[DRMB200_MAX_LINKS];        // axis code of the link of step k (un-permutation before the quaternion)
-    int8_t root_ee[MT_MAX_EE];
-    int8_t cslot[MT_MAX_EE][DRMB200_MAX_LINKS];   // per end effector and Jacobian column: joint scratch slot, or -1 (off the path)
-    uint16_t tab_map[DRMB200_MAX_LINKS * 12];     // canonical (F~, r~) entry i of step k = i / 12 (see PathProgram)
-};
 
 struct MtArgs {
     const float* __restrict__ table;
@@ -343,7 +323,7 @@ fk_tree_kernel(const __grid_constant__ MultiProgram prog, const MtArgs args) {
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-static int build_multi_program(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, MultiProgram* prog) {
+int build_multi_program(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, MultiProgram* prog) {
     if (topo == nullptr || ee_links == nullptr) { set_error("topology / ee_links is null"); return DRMB200_EINVAL; }
     const int N = topo->n_links;
     if (N < 1 || N > DRMB200_MAX_LINKS) { set_error("n_links=%d outside [1, %d]", N, DRMB200_MAX_LINKS); return DRMB200_ELIMIT; }

@@ -94,6 +94,11 @@ _SIGNATURES = {
                                                   _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int32,
                                                   ctypes.c_float, ctypes.c_float, ctypes.c_float, _c_float_p, _c_float_p,
                                                   _c_float_p, ctypes.c_void_p, _c_float_p, ctypes.c_void_p]),
+    "drmb200_inverse_kinematics_multi": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                                        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                        _c_float_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_float,
+                                                        ctypes.c_float, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
+                                                        _c_float_p, ctypes.c_void_p]),
     "drmb200_kinematic_state": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
                                                _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table": (ctypes.c_int, [_c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_void_p]),
@@ -386,6 +391,36 @@ def inverse_kinematics_raw(topo, ee_link, table, q0, target_pos, target_quat=Non
                                               _ptr(q), _ptr(pos_err), _ptr(rot_err), _ptr(converged), _ptr(damping_out),
                                               _stream())
     _check(rc, "drmb200_inverse_kinematics")
+    return q, pos_err, rot_err, converged.view(torch.bool), damping_out
+
+
+def inverse_kinematics_multi_raw(topo, ee_links, table, q0, target_pos, target_quat=None, lower=None, upper=None, damping=None,
+                                 max_iters=100, damping_init=IK_DAMPING_INIT, pos_tol=1e-4, rot_tol=1e-3):
+    """Levenberg-Marquardt inverse kinematics of several links at once, one solve over their stacked errors, all iterations
+    in one launch (drmb200_inverse_kinematics_multi).  q0 [B, n], target_pos [n_ee, B, 3], target_quat [n_ee, B, 4] xyzw or
+    None (position only), lower / upper [n] or None, damping [B] or None.  Returns (q [B, n], pos_err [n_ee, B],
+    rot_err [n_ee, B], converged [B] bool, damping [B])."""
+    _require_cuda(table, q0, target_pos, target_quat, lower, upper, damping)
+    q0, target_pos = q0.contiguous(), target_pos.contiguous()
+    target_quat = None if target_quat is None else target_quat.contiguous()
+    lower = None if lower is None else lower.contiguous()
+    upper = None if upper is None else upper.contiguous()
+    damping = None if damping is None else damping.contiguous()
+    B, n = q0.shape
+    dev, E = q0.device, len(ee_links)
+    q = torch.empty((B, n), device=dev, dtype=torch.float32)
+    pos_err = torch.empty((E, B), device=dev, dtype=torch.float32)
+    rot_err = torch.empty((E, B), device=dev, dtype=torch.float32)
+    converged = torch.empty(B, device=dev, dtype=torch.uint8)
+    damping_out = torch.empty(B, device=dev, dtype=torch.float32)
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    with _on(dev):
+        rc = lib().drmb200_inverse_kinematics_multi(ctypes.byref(topo), E, links, _ptr(table), _ptr(q0), _ptr(target_pos),
+                                                    _ptr(target_quat), _ptr(lower), _ptr(upper), _ptr(damping), B,
+                                                    int(max_iters), ctypes.c_float(damping_init), ctypes.c_float(pos_tol),
+                                                    ctypes.c_float(rot_tol), _ptr(q), _ptr(pos_err), _ptr(rot_err),
+                                                    _ptr(converged), _ptr(damping_out), _stream())
+    _check(rc, "drmb200_inverse_kinematics_multi")
     return q, pos_err, rot_err, converged.view(torch.bool), damping_out
 
 

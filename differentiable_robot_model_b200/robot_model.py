@@ -83,7 +83,9 @@ def tensor_check(function):
 class InverseKinematicsResult(NamedTuple):
     """What :meth:`DifferentiableRobotModel.compute_inverse_kinematics` returns, per row: the joint angles, the position
     and orientation errors at them (metres / radians; orientation 0 for position-only solves), whether both are within
-    tolerance, and the final Levenberg-Marquardt damping (pass it back as ``damping`` to continue a solve)."""
+    tolerance, and the final Levenberg-Marquardt damping (pass it back as ``damping`` to continue a solve).
+    :meth:`DifferentiableRobotModel.compute_inverse_kinematics_multi` returns the same with the errors per link,
+    [n_links x batch_size]."""
     q: torch.Tensor
     pos_error: torch.Tensor
     rot_error: torch.Tensor
@@ -517,6 +519,67 @@ class DifferentiableRobotModel(torch.nn.Module):
             None if target_quat is None else target_quat.detach(), lower, upper,
             None if damping is None else damping[:, 0], max_iters, damping_init, pos_tol, rot_tol)
         return q, pos_err, rot_err, converged, damp
+
+    def compute_inverse_kinematics_multi(
+        self,
+        q0: torch.Tensor,
+        link_names: List[str],
+        target_pos: torch.Tensor,
+        target_quat: Optional[torch.Tensor] = None,
+        max_iters: int = 100,
+        pos_tol: float = 1e-4,
+        rot_tol: float = 1e-3,
+        respect_joint_limits: bool = True,
+        damping: Optional[Union[float, torch.Tensor]] = None,
+    ) -> InverseKinematicsResult:
+        r"""Inverse kinematics of several links at once (e.g. the fingertips of a hand, or of a hand on an arm): up to
+        ``max_iters`` Levenberg-Marquardt iterations per row over the stacked errors of every link, all in ONE launch
+        (``csrc/inverse_kinematics_multi.cu``; the algorithm is stated in ``include/drm_b200.h``).  Joints shared by several
+        links move for all of them together, which separate :meth:`compute_inverse_kinematics` calls cannot do.
+
+        Args:
+            q0: start joint angles [batch_size x n_dofs] (clamped to the joint limits first)
+            link_names: the links (at most 8, distinct) whose frames should reach their targets
+            target_pos: target positions [n_links x batch_size x 3] (``[n_links x 3]`` for 1-D ``q0``), the layout of
+                :meth:`compute_fk_and_jacobian_multi`'s outputs stacked
+            target_quat: target orientations [n_links x batch_size x 4] xyzw (normalised here); None solves for the
+                positions only
+            pos_tol, rot_tol: a row stops once every link's position error (m) and orientation error (rad) are within these
+            respect_joint_limits: clamp every iterate to :meth:`get_joint_limits`
+            damping: initial damping, a float or one value per row [batch_size]; None: 1e-2
+        Returns: :class:`InverseKinematicsResult` ``(q, pos_error, rot_error, converged, damping)`` with ``pos_error`` and
+        ``rot_error`` [n_links x batch_size]; squeezed for 1-D ``q0``.  Joints on none of the root -> link paths are returned
+        unchanged.  The outputs carry no autograd graph: they use the current values of the link parameters (learnable and
+        fused ones included) but are not differentiable."""
+        links = [self._name_to_idx_map[name] for name in link_names]      # KeyError for unknown links
+        E = len(links)
+        squeeze = q0.ndim == 1
+        damping_init = engine.IK_DAMPING_INIT
+        per_row = None
+        if isinstance(damping, torch.Tensor):
+            per_row = damping.detach()
+        elif damping is not None:
+            damping_init = float(damping)
+        for t in (q0, target_pos, target_quat, per_row):
+            assert t is None or t.device.type == self._device.type, f"Input argument of different device as module: {t}"
+        if squeeze:
+            q0, target_pos = q0.unsqueeze(0), target_pos.unsqueeze(1)
+            target_quat = None if target_quat is None else target_quat.unsqueeze(1)
+            per_row = None if per_row is None else per_row.reshape(1)
+        self._check_q(q0)
+        B = q0.shape[0]
+        assert target_pos.shape == (E, B, 3), "target_pos must be [n_links x batch_size x 3]"
+        assert target_quat is None or target_quat.shape == (E, B, 4), "target_quat must be [n_links x batch_size x 4]"
+        assert per_row is None or per_row.shape == (B,), "damping must be a float or [batch_size]"
+        lower, upper = self._joint_limit_tensors() if respect_joint_limits else (None, None)
+        out = engine.inverse_kinematics_multi_raw(
+            self._topology, links, self._link_table().detach(), q0.detach(), target_pos.detach(),
+            None if target_quat is None else target_quat.detach(), lower, upper, per_row, int(max_iters), damping_init,
+            float(pos_tol), float(rot_tol))
+        if squeeze:
+            q, pos_err, rot_err, converged, damp = out
+            out = (q[0], pos_err[:, 0], rot_err[:, 0], converged[0], damp[0])
+        return InverseKinematicsResult(*out)
 
     def _joint_limit_tensors(self):
         """(lower, upper) [n_dofs] fp32 on the model's device, from get_joint_limits(), built once."""

@@ -24,6 +24,7 @@
  *                                        q, qd (and f), [B, n, n] each, one launch (the reference: autograd, row by row).
  *   drmb200_inverse_kinematics           Levenberg-Marquardt inverse kinematics of one link for a batch of pose targets,
  *                                        all iterations in one launch (the reference has no IK).
+ *   drmb200_inverse_kinematics_multi     the same for several links at once (one solve over their stacked errors).
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -335,6 +336,41 @@ int drmb200_inverse_kinematics(const drmb200_topology_t* topo, int32_t ee_link, 
                                int64_t batch, int32_t max_iters, float damping_init, float pos_tol, float rot_tol,
                                float* q, float* pos_err, float* rot_err, uint8_t* converged, float* damping_out,
                                void* cuda_stream);
+
+/*
+ * Inverse kinematics of SEVERAL links at once (fingertips of a hand, an arm and its hand): one Levenberg-Marquardt solve over
+ * the stacked errors of every link per row, all iterations in ONE launch (csrc/inverse_kinematics_multi.cu).  The links share
+ * the joints on the common part of their root paths, so they are moved together, which no set of single-link solves does.
+ *   ee_links [n_ee]  host array of distinct link indices, 1 <= n_ee <= 8, each with a movable joint on its root path.
+ *   U = the movable joints on the union of the root -> link paths, n_u = |U|; M = 3 n_ee (position) or 6 n_ee (pose).
+ * Per row b, in fp32:
+ *   q <- clamp(q0[b]) and lambda <- damping_in[b] (damping_init when NULL), as drmb200_inverse_kinematics; evaluate at q:
+ *   for every link e its pose and Jacobian (as drmb200_fk_jacobian_multi returns them) and its errors e_pos,e and e_rot,e
+ *   (as drmb200_inverse_kinematics computes them: normalised target, w < 0 flip, atan2 rotation vector).  e and J [M, n_u]
+ *   are stacked link by link: rows [6e, 6e + 3) position, [6e + 3, 6e + 6) rotation (3 position rows per link for position
+ *   only).  E = sum over e in link order of (|e_pos,e|^2 + |e_rot,e|^2); done = every link has |e_pos,e| <= pos_tol and
+ *   |e_rot,e| <= rot_tol.
+ *   max_iters times, skipping rows that are done, one damped least-squares step in the smaller space:
+ *     M <= n_u (task space):  A = J J^T + lambda I_M,   dq = J^T A^-1 e;
+ *     M >  n_u (joint space): A = J^T J + lambda I_nu,  dq = A^-1 J^T e   (equal to the above: push-through identity);
+ *   Cholesky of A with the rejection rule of drmb200_inverse_kinematics; q' = clamp(q + dq) on U, evaluated as above; accept
+ *   iff E' < E, with the same damping update (halve, floor 1e-5 / times 4, cap 1e5).
+ * Outputs at the returned q: q [B, n_dofs], pos_err / rot_err [n_ee, B] (rot_err = 0 for position only), converged [B] and
+ * damping_out [B].  K iterations in one call are bit-identical to K calls with max_iters = 1 that pass q and damping_out on;
+ * with n_ee = 1 and M <= n_u the result is bit-identical to drmb200_inverse_kinematics of that link.  Joints outside U never
+ * move.  Inputs: q0 [B, n_dofs], target_pos [n_ee, B, 3], target_quat [n_ee, B, 4] or NULL (the [n_ee, B, ...] blocks of
+ * drmb200_fk_jacobian_multi, so its output at a goal configuration is a valid target), lower / upper [n_dofs] (both or
+ * neither), damping_in [B] or NULL.  Device pointers, caller-allocated outputs that must not alias inputs; no allocation,
+ * no synchronisation (graph-capturable).  batch == 0 is a no-op.  DRMB200_ELIMIT for n_ee outside [1, 8] or when a one-row
+ * CTA needs more than 227 KB of shared memory; DRMB200_EINVAL for a link requested twice, a link without a movable joint on
+ * its root path (the root included) and the argument errors of drmb200_inverse_kinematics.
+ */
+int drmb200_inverse_kinematics_multi(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links,
+                                     const float* table, const float* q0, const float* target_pos,
+                                     const float* target_quat, const float* lower, const float* upper,
+                                     const float* damping_in, int64_t batch, int32_t max_iters, float damping_init,
+                                     float pos_tol, float rot_tol, float* q, float* pos_err, float* rot_err,
+                                     uint8_t* converged, float* damping_out, void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state
