@@ -112,6 +112,8 @@ int inverse_kinematics_device(const drmb200_topology_t*, int32_t, const float*, 
 int inverse_kinematics_multi_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
                                     const float*, const float*, const float*, const float*, int64_t, int32_t, float, float, float,
                                     float*, float*, float*, uint8_t*, float*, cudaStream_t);
+int operational_space_dynamics_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                                      const float*, int64_t, uint32_t, int32_t, float*, float*, float*, float*, cudaStream_t);
 int64_t table_grad_workspace_bytes(const drmb200_topology_t*, int64_t);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 int mass_matrix_device(const drmb200_topology_t*, const float*, const float*, int64_t, float*, cudaStream_t);
@@ -433,6 +435,15 @@ int drmb200_inverse_kinematics_multi(const drmb200_topology_t* topo, int32_t n_e
     return drm::inverse_kinematics_multi_device(topo, n_ee, ee_links, table, q0, target_pos, target_quat, lower, upper, damping_in,
                                                 batch, max_iters, damping_init, pos_tol, rot_tol, q, pos_err, rot_err, converged,
                                                 damping_out, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                       const float* q, const float* qd, const float* f, int64_t batch, uint32_t flags,
+                                       int32_t position_only, float* inv_inertia, float* acceleration, float* velocity,
+                                       float* bias_acceleration, void* cuda_stream) {
+    return drm::operational_space_dynamics_device(topo, n_ee, ee_links, table, q, qd, f, batch, flags, position_only, inv_inertia,
+                                                  acceleration, velocity, bias_acceleration,
+                                                  static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_kinematic_state(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -1,0 +1,411 @@
+// operational_space.cu -- batched operational-space dynamics of several links (sm_90a).
+//
+// Per row (q, qd, f) and a list of E links, in ONE launch (spec in include/drm_b200.h and DESIGN.md §3):
+//   J               [M, n]  the links' geometric Jacobians stacked (6 rows per link: linear over angular; 3 for position only)
+//   inv_inertia     [M, M]  J G J^T, G[:, j] = forward dynamics at (q, 0, e_j) without gravity or damping (dqdd_df)
+//   velocity        [M]     J qd
+//   bias            [M]     Jdot qd: the link origins' classical accelerations (and angular accelerations) at qdd = 0
+//   acceleration    [M]     J qdd + Jdot qd, qdd = forward dynamics at (q, qd, f) with the call's flags
+//
+// One thread per row.  Three parts share the row's shared-memory state:
+//   * kinematics: one depth-first walk of the union of the root -> link paths (the MultiProgram of multi_program.cuh, in the
+//     canonical +z frames, unfolded, so links behind fixed joints work).  Along the walk it propagates, besides (R, p), the
+//     angular velocity omega, the origin velocity v, and at qdd = 0 the angular acceleration alpha and the origin's
+//     classical acceleration a, all in the world frame:  with d = R_parent r_i,
+//         v_i = v_p + omega_p x d,   a_i = a_p + alpha_p x d + omega_p x (omega_p x d),
+//     then at a joint with world axis z and rate qd:  alpha += qd omega x z,  omega += qd z.
+//     At link e, J qd = (v_e; omega_e) and Jdot qd = (a_e; alpha_e) -- the same quantities as
+//     sum_j qd_j [(omega_j x z_j) x (p_e - p_j) + z_j x (v_e - v_j);  omega_j x z_j], but every term is a short local
+//     vector, so nothing cancels when the links are far from the world origin.  The state is spilled at branch points.
+//   * forward dynamics: aba_body.cuh on the whole (unfolded) tree gives qdd and leaves, per link, cos / sin of the joint angle,
+//     U and d of the articulated inertia.  Those depend on q only, so every further right-hand side tau is two O(n) sweeps of
+//     6-vectors at zero velocity and zero gravity, with the articulated-body arithmetic of aba_body (the tangent of its passes
+//     2 and 3 in f):  leaves -> root  u = tau - p_z, pa = p + U u / (d + eps), p_parent += X^T pa;
+//                     root -> leaves  a' = X a_parent, x = (u - U . a') / d, a = a' + e_z x.
+//   * the product is formed in the smaller space (U = the movable joints on the union of the paths, n_u of them):
+//         M <= n_u:  M sweeps with tau = J^T e_k give the columns of G J^T, then inv_inertia[:, k] = J (G J^T e_k);
+//         M >  n_u:  n_u sweeps with tau = e_j give the columns G e_j, then inv_inertia += (J G e_j) J[:, j]^T.
+//
+// Shared memory, per row and slot-major (element e of row t at base[e * T + t]) except the ABA's q / qd / f / qdd rows
+// (AbaSmemLayout): the ABA link and branch state, J [M][n_u], the walk's joint scratch (z, z x p per path depth) and spilled
+// branch state (R, p, omega, v, alpha, a: 24 floats), and the output tiles inv_inertia [M][M], velocity, bias and acceleration
+// [M].  The output tiles are written back with a cooperative transposing copy: consecutive threads store consecutive floats
+// of the contiguous [T, M, M] block, so the stores coalesce without a second row-major copy of the tile in shared memory.
+#include "aba_body.cuh"
+#include "multi_program.cuh"
+
+namespace drm {
+
+constexpr int OSD_STATE = 24;          // floats of a spilled branch state: R (9), p, omega, v, alpha, a
+
+struct OsdProgram {
+    MultiProgram walk;
+    int32_t n_u;                       // movable joints on the union of the paths
+    int8_t u_dof[DRMB200_MAX_LINKS];   // U column -> q / dof column, in walk order
+};
+
+struct OsdArgs {
+    const float* __restrict__ table;
+    const float* __restrict__ q;
+    const float* __restrict__ qd;
+    const float* __restrict__ f;
+    float* __restrict__ inv_inertia;   // [B, M, M] or null
+    float* __restrict__ acceleration;  // [B, M] or null
+    float* __restrict__ velocity;      // [B, M] or null
+    float* __restrict__ bias;          // [B, M] or null
+    int64_t batch;
+    uint32_t flags;
+    int32_t M;                         // rows: 6 n_ee (pose) or 3 n_ee (position only)
+    int32_t aligned;
+};
+
+struct OsdSmemLayout {
+    AbaSmemLayout aba;
+    int jac, jscr, state, vel, bias, acc, inv, total_floats;
+    __host__ __device__ OsdSmemLayout(int T, const TreeProgram& tp, const OsdProgram& P, int M)
+        : aba(T, tp.n_dofs, tp.n_links, tp.n_slots) {
+        int o = aba.total_floats;
+        jac = o;   o += M * P.n_u * T;
+        jscr = o;  o += 6 * P.walk.n_jslots * T;
+        state = o; o += OSD_STATE * P.walk.n_state_slots * T;
+        vel = o;   o += M * T;
+        bias = o;  o += M * T;
+        acc = o;   o += M * T;
+        inv = o;   o += M * M * T;
+        total_floats = o;
+    }
+};
+
+// The kinematic walk of one row: J [M][n_u], velocity and bias [M] (this row's slot-major slots; entries of links that are
+// not walked -- the root -- and of joints off a link's path are left as staged: zero).  qrow / qdrow: the row's q, qd.
+template <int T>
+__device__ __forceinline__ void osd_walk(const OsdProgram& P, const float* s_tab, const float* qrow, const float* qdrow, int MR,
+                                         float* J, float* vel, float* bias, float* jscr, float* st) {
+    const MultiProgram& W = P.walk;
+    const int n_u = P.n_u;
+    const int rs = n_u * T;                  // stride between rows of J
+    const V3 zero = v3(0.f, 0.f, 0.f);
+    M3 R = identity3();
+    V3 p = zero, w = zero, v = zero, A = zero, a = zero;
+    for (int k = 0; k < W.n_steps; ++k) {
+        M3 F; V3 r;
+        load_Fr(s_tab + (int)W.link[k] * DRMB200_TABLE_STRIDE, F, r);
+        const int src = W.psrc[k];
+        if (src < 0) {
+            R = identity3(); p = w = v = A = a = zero;
+        } else if (src > 0) {
+            const float* s = st + (src - 1) * OSD_STATE * T;
+            R = ldm(s, T); p = ldv(s + 9 * T, T); w = ldv(s + 12 * T, T); v = ldv(s + 15 * T, T);
+            A = ldv(s + 18 * T, T); a = ldv(s + 21 * T, T);
+        }
+        const V3 d = mul(R, r);              // parent origin -> this origin, world frame, on the parent body
+        p = p + d;
+        v = cross_add(w, d, v);              // v_i = v_p + w_p x d
+        a = a + cross_add(A, d, cross(w, cross(w, d)));     // a_i = a_p + A_p x d + w_p x (w_p x d)
+        R = mul(R, F);
+        const int c = W.dof[k];
+        if (c >= 0) {
+            float sn, cs;
+            sincos_pi2(qrow[c], sn, cs);
+            const V3 z = col2(R);            // joint axis in the world frame (unchanged by Rz)
+            float* js = jscr + W.jslot[k] * 6 * T;
+            stv(js, T, z);
+            stv(js + 3 * T, T, cross(z, p));
+            const float qd = qdrow[c];
+            A = A + qd * cross(w, z);        // + qd dz/dt
+            w = w + qd * z;
+            rotate_z(R, cs, sn);
+        }
+        const int sv = W.save[k];
+        if (sv >= 0) {
+            float* s = st + sv * OSD_STATE * T;
+            stm(s, T, R); stv(s + 9 * T, T, p); stv(s + 12 * T, T, w); stv(s + 15 * T, T, v);
+            stv(s + 18 * T, T, A); stv(s + 21 * T, T, a);
+        }
+        const int l = W.ee[k];
+        if (l < 0) continue;
+        // link l: its rows of J (J_lin = z x p_e - z x p_j over J_ang = z), of J qd and of Jdot qd
+        float* Jl = J + MR * l * rs;
+        for (int u = 0; u < n_u; ++u) {
+            const int s = W.cslot[l][P.u_dof[u]];
+            if (s < 0) continue;             // off this link's path: stays zero
+            const float* js = jscr + s * 6 * T;
+            const V3 z = ldv(js, T), m = ldv(js + 3 * T, T);
+            const V3 j = cross_add(z, p, v3(-m.x, -m.y, -m.z));
+            float* col = Jl + u * T;
+            col[0] = j.x; col[rs] = j.y; col[2 * rs] = j.z;
+            if (MR == 6) { col[3 * rs] = z.x; col[4 * rs] = z.y; col[5 * rs] = z.z; }
+        }
+        stv(vel + MR * l * T, T, v);
+        stv(bias + MR * l * T, T, a);
+        if (MR == 6) { stv(vel + (MR * l + 3) * T, T, w); stv(bias + (MR * l + 3) * T, T, A); }
+    }
+}
+
+// x = G tau for one row: passes 2 and 3 of aba_body at zero velocity and gravity, on the U, d, cos, sin that aba_body left
+// in the row's link slots (lk0).  tau / x: the row's n floats (row-major, like the ABA's f / qdd rows); sl0: its branch slots.
+// Each link's u is kept in the slot aba_body used for its own u (dead once aba_body returned).
+template <int T>
+__device__ __forceinline__ void aba_unit_response(const TreeProgram& prog, const float* s_tab, const float* tau, float* x,
+                                                  float* lk0, float* sl0) {
+    const int N = prog.n_links;
+    const V3 zero = v3(0.f, 0.f, 0.f);
+    {   // leaves -> root
+        V3 c_ang = zero, c_lin = zero;
+        for (int i = N - 1; i >= 1; --i) {
+            float* lk = lk0 + i * ABA_LINK * T;
+            V3 p_ang = zero, p_lin = zero;
+            if (i + 1 < N && prog.psrc[i + 1] == 0) { p_ang = c_ang; p_lin = c_lin; }
+            const int sv = prog.save[i];
+            if (sv >= 0) {
+                const float* sl = sl0 + sv * ABA_SLOT * T;
+                p_ang = p_ang + ldv(sl + 36 * T, T); p_lin = p_lin + ldv(sl + 39 * T, T);
+            }
+            const int c = prog.dof[i];
+            float u = 0.f;
+            if (c >= 0) u = tau[c] - p_ang.z;
+            const int Pi = prog.parent[i];
+            if (Pi > 0) {
+                V3 pa_ang = p_ang, pa_lin = p_lin;
+                M3 M; V3 r;
+                load_Fr(s_tab + i * DRMB200_TABLE_STRIDE, M, r);
+                if (c >= 0) {
+                    const float ud = u * (1.f / (lk[13 * T] + ABA_EPS));
+                    pa_ang = pa_ang + ud * ldv(lk + 6 * T, T);
+                    pa_lin = pa_lin + ud * ldv(lk + 9 * T, T);
+                    rotate_z(M, lk[0], lk[T]);
+                }
+                const V3 q_lin = mul(M, pa_lin);                       // force transform X^T
+                const V3 q_ang = cross_add(r, q_lin, mul(M, pa_ang));
+                if (Pi == i - 1) { c_ang = q_ang; c_lin = q_lin; }
+                else {
+                    float* sl = sl0 + (int)prog.save[Pi] * ABA_SLOT * T;
+                    if (prog.accw[i] != 2) {
+                        stv(sl + 36 * T, T, ldv(sl + 36 * T, T) + q_ang); stv(sl + 39 * T, T, ldv(sl + 39 * T, T) + q_lin);
+                    } else {
+                        stv(sl + 36 * T, T, q_ang); stv(sl + 39 * T, T, q_lin);
+                    }
+                }
+            }
+            lk[12 * T] = u;
+        }
+    }
+    {   // root -> leaves
+        V3 al = zero, a = zero;
+        for (int i = 1; i < N; ++i) {
+            M3 M; V3 r;
+            load_Fr(s_tab + i * DRMB200_TABLE_STRIDE, M, r);
+            const float* lk = lk0 + i * ABA_LINK * T;
+            const int src = prog.psrc[i];
+            V3 alp, ap;
+            if (src == 0) { alp = al; ap = a; }
+            else if (src < 0) { alp = zero; ap = zero; }
+            else { const float* sl = sl0 + (src - 1) * ABA_SLOT * T; alp = ldv(sl, T); ap = ldv(sl + 3 * T, T); }
+            const int c = prog.dof[i];
+            if (c >= 0) rotate_z(M, lk[0], lk[T]);
+            al = mulT(M, alp);
+            a = mulT(M, cross_add(alp, r, ap));
+            if (c >= 0) {
+                const V3 Ua = ldv(lk + 6 * T, T), Ul = ldv(lk + 9 * T, T);
+                const float u = lk[12 * T], d = lk[13 * T];
+                const float xc = (1.0f / d) * (u - (dot(Ua, al) + dot(Ul, a)));
+                x[c] = xc;
+                al.z += xc;
+            }
+            const int sv = prog.save[i];
+            if (sv >= 0) { float* sl = sl0 + sv * ABA_SLOT * T; stv(sl, T, al); stv(sl + 3 * T, T, a); }
+        }
+    }
+}
+
+// slot-major shared tile [e][T] -> contiguous global block [valid][per_row]
+__device__ __forceinline__ void store_transposed(float* dst, const float* src, int per_row, int valid, int T) {
+    const int total = valid * per_row;
+    for (int i = threadIdx.x; i < total; i += blockDim.x) {
+        const int r = i / per_row, e = i - r * per_row;
+        dst[i] = src[e * T + r];
+    }
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+operational_space_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ OsdProgram P, const OsdArgs args) {
+    extern __shared__ __align__(128) float smem[];
+    __shared__ __align__(8) uint64_t mbar;
+
+    const int n = prog.n_dofs;
+    const int M = args.M;
+    const int MR = M / P.walk.n_ee;
+    const int n_u = P.n_u;
+    const OsdSmemLayout L(T, prog, P, M);
+    float* s_q = smem + L.aba.q;
+    float* s_qd = smem + L.aba.qd;
+    float* s_f = smem + L.aba.f;
+    float* s_qdd = smem + L.aba.qdd;
+    float* s_tab = smem + L.aba.table;
+
+    const int tid = threadIdx.x;
+    const int64_t tile_start = (int64_t)blockIdx.x * T;
+    const int valid = (int)min((int64_t)T, args.batch - tile_start);
+    const bool vec_ok = args.aligned;
+    const bool bulk = args.aligned && n > 0 && ((valid & 3) == 0);
+
+    if (bulk) {
+        if (tid == 0) {
+            mbar_init(&mbar, 1);
+            fence_mbar_init();
+            const uint32_t bytes = (uint32_t)valid * n * 4u;
+            mbar_arrive_expect_tx(&mbar, 3u * bytes);
+            bulk_g2s(s_q, args.q + tile_start * n, bytes, &mbar);
+            bulk_g2s(s_qd, args.qd + tile_start * n, bytes, &mbar);
+            bulk_g2s(s_f, args.f + tile_start * n, bytes, &mbar);
+        }
+    } else {
+        coop_copy(s_q, args.q + tile_start * n, valid * n, vec_ok);
+        coop_copy(s_qd, args.qd + tile_start * n, valid * n, vec_ok);
+        coop_copy(s_f, args.f + tile_start * n, valid * n, vec_ok);
+    }
+    stage_canonical_table(s_tab, args.table, prog, T);
+    // J, velocity and bias start at zero: rows of links that are not walked (the root) and columns off a link's path
+    for (int i = L.jac + tid; i < L.jscr; i += T) smem[i] = 0.f;
+    for (int i = L.vel + tid; i < L.acc; i += T) smem[i] = 0.f;
+    __syncthreads();
+    if (bulk) mbar_wait(&mbar, 0);
+
+    if (tid < valid) {
+        const float* qrow = s_q + tid * n;
+        const float* qdrow = s_qd + tid * n;
+        float* frow = s_f + tid * n;
+        float* qddrow = s_qdd + tid * n;
+        float* lk0 = smem + L.aba.link + tid;
+        float* sl0 = smem + L.aba.slots + tid;
+        float* J = smem + L.jac + tid;
+        float* vel = smem + L.vel + tid;
+        float* bias = smem + L.bias + tid;
+        float* acc = smem + L.acc + tid;
+        float* inv = smem + L.inv + tid;
+        const int rs = n_u * T;
+        osd_walk<T>(P, s_tab, qrow, qdrow, MR, J, vel, bias, smem + L.jscr + tid, smem + L.state + tid);
+        if (args.acceleration != nullptr || args.inv_inertia != nullptr) {
+            aba_body<T>(prog, s_tab, qrow, qdrow, frow, qddrow, lk0, sl0, args.flags);
+            for (int m = 0; m < M; ++m) {           // J qdd + Jdot qd
+                float s = bias[m * T];
+                for (int u = 0; u < n_u; ++u) s = fmaf(J[m * rs + u * T], qddrow[P.u_dof[u]], s);
+                acc[m * T] = s;
+            }
+        }
+        if (args.inv_inertia != nullptr) {
+            if (M <= n_u) {
+                for (int k = 0; k < M; ++k) {       // column k: J G J^T e_k
+                    for (int c = 0; c < n; ++c) frow[c] = 0.f;
+                    for (int u = 0; u < n_u; ++u) frow[P.u_dof[u]] = J[k * rs + u * T];
+                    aba_unit_response<T>(prog, s_tab, frow, qddrow, lk0, sl0);
+                    for (int m = 0; m < M; ++m) {
+                        float s = 0.f;
+                        for (int u = 0; u < n_u; ++u) s = fmaf(J[m * rs + u * T], qddrow[P.u_dof[u]], s);
+                        inv[(m * M + k) * T] = s;
+                    }
+                }
+            } else {
+                for (int i = 0; i < M * M; ++i) inv[i * T] = 0.f;
+                for (int j = 0; j < n_u; ++j) {     // += (J G e_j) J[:, j]^T
+                    for (int c = 0; c < n; ++c) frow[c] = 0.f;
+                    frow[P.u_dof[j]] = 1.f;
+                    aba_unit_response<T>(prog, s_tab, frow, qddrow, lk0, sl0);
+                    for (int m = 0; m < M; ++m) {
+                        float y = 0.f;
+                        for (int u = 0; u < n_u; ++u) y = fmaf(J[m * rs + u * T], qddrow[P.u_dof[u]], y);
+                        for (int k = 0; k < M; ++k) inv[(m * M + k) * T] = fmaf(y, J[k * rs + j * T], inv[(m * M + k) * T]);
+                    }
+                }
+            }
+        }
+    }
+    __syncthreads();
+    if (args.inv_inertia != nullptr) store_transposed(args.inv_inertia + tile_start * M * M, smem + L.inv, M * M, valid, T);
+    if (args.acceleration != nullptr) store_transposed(args.acceleration + tile_start * M, smem + L.acc, M, valid, T);
+    if (args.velocity != nullptr) store_transposed(args.velocity + tile_start * M, smem + L.vel, M, valid, T);
+    if (args.bias != nullptr) store_transposed(args.bias + tile_start * M, smem + L.bias, M, valid, T);
+}
+
+// ---------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------
+template <int T>
+static int launch_osd_tile(const TreeProgram& prog, const OsdProgram& P, const OsdArgs& args, size_t smem_bytes,
+                           cudaStream_t stream) {
+    auto kern = operational_space_kernel<T>;
+    static size_t configured_by_dev[64] = {0};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    size_t& configured = configured_by_dev[dev & 63];
+    if (smem_bytes > configured) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
+        configured = smem_bytes;
+    }
+    const int64_t tiles = (args.batch + T - 1) / T;
+    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
+    kern<<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, P, args);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("operational-space dynamics launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
+    count_launch();
+    return DRMB200_OK;
+}
+
+int operational_space_dynamics_device(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                      const float* q, const float* qd, const float* f, int64_t batch, uint32_t flags,
+                                      int32_t position_only, float* inv_inertia, float* acceleration, float* velocity,
+                                      float* bias_acceleration, cudaStream_t stream) {
+    if (n_ee < 1 || n_ee > MT_MAX_EE) { set_error("n_ee=%d outside [1, %d]", n_ee, MT_MAX_EE); return DRMB200_EINVAL; }
+    if (ee_links == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
+    OsdProgram P;
+    int rc = build_multi_program(topo, n_ee, ee_links, &P.walk);
+    if (rc != DRMB200_OK) return rc;
+    const CachedPrograms* cp = cached_programs(topo, &rc);
+    if (cp == nullptr) return rc;
+    const TreeProgram& prog = cp->full;         // unfolded: the walk and the ABA share one staged canonical table
+    if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
+    if (inv_inertia == nullptr && acceleration == nullptr && velocity == nullptr && bias_acceleration == nullptr) return DRMB200_OK;
+    if (batch == 0) return DRMB200_OK;
+    // q, qd, f may be null only for a model without movable joints (empty tensors): they are then never read
+    if (table == nullptr || (prog.n_dofs > 0 && (q == nullptr || qd == nullptr || f == nullptr))) {
+        set_error("null pointer argument");
+        return DRMB200_EINVAL;
+    }
+    const MultiProgram& W = P.walk;
+    P.n_u = 0;
+    for (int k = 0; k < W.n_steps; ++k)
+        if (W.dof[k] >= 0) P.u_dof[P.n_u++] = W.dof[k];
+
+    OsdArgs args;
+    args.table = table; args.q = q; args.qd = qd; args.f = f;
+    args.inv_inertia = inv_inertia; args.acceleration = acceleration; args.velocity = velocity; args.bias = bias_acceleration;
+    args.batch = batch; args.flags = flags & (DRMB200_GRAVITY | DRMB200_DAMPING);
+    args.M = (position_only ? 3 : 6) * n_ee;
+    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+    args.aligned = (al16(q) && al16(qd) && al16(f)) ? 1 : 0;
+
+    // the largest power-of-two tile <= 64 rows while two CTAs still fit an SM, else down to one row per CTA
+    auto bytes_of = [&](int T) { return (size_t)OsdSmemLayout(T, prog, P, args.M).total_floats * sizeof(float); };
+    constexpr size_t STATIC_BYTES = 128;        // static shared memory of every instantiation (-Xptxas -v)
+    int T = 64;
+    while (T > 1 && bytes_of(T) + STATIC_BYTES > 113 * 1024) T >>= 1;
+    const size_t smem_bytes = bytes_of(T);
+    if (smem_bytes + STATIC_BYTES > 227 * 1024) {
+        set_error("operational-space dynamics needs %zu B of shared memory per CTA (> 227 KB) for one row (%d joints, %d links, M = %d)",
+                  smem_bytes + STATIC_BYTES, prog.n_dofs, prog.n_links, args.M);
+        return DRMB200_ELIMIT;
+    }
+    switch (T) {
+        case 64: return launch_osd_tile<64>(prog, P, args, smem_bytes, stream);
+        case 32: return launch_osd_tile<32>(prog, P, args, smem_bytes, stream);
+        case 16: return launch_osd_tile<16>(prog, P, args, smem_bytes, stream);
+        case 8: return launch_osd_tile<8>(prog, P, args, smem_bytes, stream);
+        case 4: return launch_osd_tile<4>(prog, P, args, smem_bytes, stream);
+        case 2: return launch_osd_tile<2>(prog, P, args, smem_bytes, stream);
+        default: return launch_osd_tile<1>(prog, P, args, smem_bytes, stream);
+    }
+}
+
+}  // namespace drm

@@ -99,6 +99,10 @@ _SIGNATURES = {
                                                         _c_float_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_float,
                                                         ctypes.c_float, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
                                                         _c_float_p, ctypes.c_void_p]),
+    "drmb200_operational_space_dynamics": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32,
+                                                          ctypes.POINTER(ctypes.c_int32), _c_float_p, _c_float_p, _c_float_p,
+                                                          _c_float_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_int32,
+                                                          _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_kinematic_state": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
                                                _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table": (ctypes.c_int, [_c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_void_p]),
@@ -422,6 +426,29 @@ def inverse_kinematics_multi_raw(topo, ee_links, table, q0, target_pos, target_q
                                                     _ptr(converged), _ptr(damping_out), _stream())
     _check(rc, "drmb200_inverse_kinematics_multi")
     return q, pos_err, rot_err, converged.view(torch.bool), damping_out
+
+
+def operational_space_dynamics_raw(topo, ee_links, table, q, qd, f, flags, position_only=False, want_inv_inertia=True,
+                                   want_acceleration=True, want_velocity=True, want_bias=True):
+    """(inv_inertia [B, M, M], acceleration [B, M], velocity [B, M], bias_acceleration [B, M]) of the links `ee_links`,
+    M = 6 len(ee_links) (3 with position_only), one launch (drmb200_operational_space_dynamics); an output not wanted is
+    None."""
+    _require_cuda(table, q, qd, f)
+    q, qd, f = q.contiguous(), qd.contiguous(), f.contiguous()
+    B = q.shape[0]
+    E = len(ee_links)
+    M = (3 if position_only else 6) * E
+    dev = q.device
+    inv = torch.empty((B, M, M), device=dev, dtype=torch.float32) if want_inv_inertia else None
+    vecs = [torch.empty((B, M), device=dev, dtype=torch.float32) if want else None
+            for want in (want_acceleration, want_velocity, want_bias)]
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    with _on(dev):
+        rc = lib().drmb200_operational_space_dynamics(ctypes.byref(topo), E, links, _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B,
+                                                      flags & 3, 1 if position_only else 0, _ptr(inv),
+                                                      *[_ptr(v) for v in vecs], _stream())
+    _check(rc, "drmb200_operational_space_dynamics")
+    return (inv, *vecs)
 
 
 def kinematic_state_raw(topo, table, q, qd=None, want_poses=True, want_quats=False):

@@ -93,6 +93,17 @@ class InverseKinematicsResult(NamedTuple):
     damping: torch.Tensor
 
 
+class OperationalSpaceDynamics(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_operational_space_dynamics` returns, per row, with M = 6 rows per link
+    (linear over angular) or 3 for position only, links stacked in the order requested: the inverse operational-space
+    inertia ``J G J^T`` [M x M], the true world-frame acceleration ``J qdd + Jdot qd`` [M], the velocity ``J qd`` [M] and
+    the bias acceleration ``Jdot qd`` [M]."""
+    inv_inertia: torch.Tensor
+    acceleration: torch.Tensor
+    velocity: torch.Tensor
+    bias_acceleration: torch.Tensor
+
+
 class DifferentiableRobotModel(torch.nn.Module):
     """Batched rigid-body kinematics / dynamics of a URDF robot on one GPU (H100, sm_90a)."""
 
@@ -466,6 +477,50 @@ class DifferentiableRobotModel(torch.nn.Module):
         table = self._link_table().detach()
         return engine.forward_dynamics_derivatives_raw(self._topology, table, q.detach(), qd.detach(), f.detach(), flags,
                                                        folded=self._folded_table())
+
+    def compute_operational_space_dynamics(
+        self,
+        q: torch.Tensor,
+        qd: torch.Tensor,
+        f: torch.Tensor,
+        link_names: List[str],
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = False,
+        position_only: bool = False,
+    ) -> OperationalSpaceDynamics:
+        r"""Operational-space dynamics of several links (at most 8, distinct) in ONE launch (``csrc/operational_space.cu``;
+        the definition is stated in ``include/drm_b200.h``).  With ``J`` the links' geometric Jacobians stacked (as
+        :meth:`compute_endeffector_jacobian` returns them, linear rows over angular rows; linear rows only with
+        ``position_only``), ``qdd`` what :meth:`compute_forward_dynamics` returns and ``G`` the ``dqdd_df`` of
+        :meth:`compute_forward_dynamics_derivatives` (``H^-1`` for symmetric inertias):
+
+        * ``inv_inertia = J G J^T``: maps a stacked force / wrench ``F`` applied at the links to their acceleration change,
+          ``acceleration(f + J^T F) = acceleration(f) + inv_inertia F``; invert it (regularised as you see fit) for the
+          operational-space inertia, or use the position-only version of several fingertips as a contact-space inverse
+          inertia;
+        * ``velocity = J qd``, ``bias_acceleration = Jdot qd`` and ``acceleration = J qdd + Jdot qd``.
+
+        Args:
+            q, qd, f: joint angles / velocities / applied joint forces [batch_size x n_dofs]
+            link_names: the links, stacked in this order; the root and links with no movable joint on their root path get
+                zero rows and columns
+            include_gravity, use_damping: as for :meth:`compute_forward_dynamics`
+            position_only: 3 rows per link (the linear ones) instead of 6
+        Returns: :class:`OperationalSpaceDynamics` with shapes [batch_size x M x M] and [batch_size x M] (``[M x M]`` and
+        ``[M]`` for 1-D inputs), M = 6 or 3 per link.  The outputs carry no autograd graph: they use the current values of
+        the link parameters (learnable and fused ones included) but are not differentiable."""
+        links = [self._name_to_idx_map[name] for name in link_names]      # KeyError for unknown links
+        assert len(set(links)) == len(links), "link names must be distinct"
+        return OperationalSpaceDynamics(*self._operational_space_dynamics(q, qd, f, links=links, include_gravity=include_gravity,
+                                                                          use_damping=use_damping, position_only=position_only))
+
+    @tensor_check
+    def _operational_space_dynamics(self, q, qd, f, links, include_gravity, use_damping, position_only):
+        self._check_q(q, qd, f)
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table().detach()
+        return engine.operational_space_dynamics_raw(self._topology, links, table, q.detach(), qd.detach(), f.detach(), flags,
+                                                     position_only=bool(position_only))
 
     def compute_inverse_kinematics(
         self,

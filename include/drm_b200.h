@@ -25,6 +25,8 @@
  *   drmb200_inverse_kinematics           Levenberg-Marquardt inverse kinematics of one link for a batch of pose targets,
  *                                        all iterations in one launch (the reference has no IK).
  *   drmb200_inverse_kinematics_multi     the same for several links at once (one solve over their stacked errors).
+ *   drmb200_operational_space_dynamics   inverse operational-space inertia J G J^T and the velocities, bias and true
+ *                                        accelerations of several links, one launch (the reference has none of these).
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -371,6 +373,35 @@ int drmb200_inverse_kinematics_multi(const drmb200_topology_t* topo, int32_t n_e
                                      const float* damping_in, int64_t batch, int32_t max_iters, float damping_init,
                                      float pos_tol, float rot_tol, float* q, float* pos_err, float* rot_err,
                                      uint8_t* converged, float* damping_out, void* cuda_stream);
+
+/*
+ * Operational-space dynamics of SEVERAL links, one launch (csrc/operational_space.cu).  Per row b, for the model, the state
+ * (q, qd), the applied joint forces f, flags (DRMB200_GRAVITY, DRMB200_DAMPING as for drmb200_forward_dynamics) and the
+ * distinct links ee_links [n_ee] (host array, 1 <= n_ee <= 8):
+ *   J [M, n_dofs]  every link's geometric Jacobian as drmb200_fk_jacobian returns it (link frame origin, world frame, the 3
+ *                  linear rows over the 3 angular rows), stacked in list order: M = 6 n_ee; position_only != 0 keeps the
+ *                  linear rows, M = 3 n_ee.  A link without a movable joint on its root path, the root included, has zero rows.
+ *   qdd            what drmb200_forward_dynamics computes at (q, qd, f) with `flags`.
+ *   G [n, n]       G[:, j] = forward dynamics at (q, 0, e_j) without gravity or damping (the dqdd_df of
+ *                  drmb200_forward_dynamics_derivatives): H^-1 for symmetric inertias; for a non-symmetric inertia matrix the
+ *                  result follows the articulated-body arithmetic, not H^-1.
+ * Outputs, caller-allocated, fp32, row-major; NULL skips one (all NULL: nothing is launched):
+ *   inv_inertia        [B, M, M]  J G J^T, off-diagonal blocks of links sharing joints included, not symmetrised
+ *   velocity           [B, M]     J qd
+ *   bias_acceleration  [B, M]     Jdot qd = sum_k d(J qd)/dq_k qd_k: the classical acceleration of each link origin (and the
+ *                                 angular acceleration) at qdd = 0
+ *   acceleration       [B, M]     J qdd + Jdot qd, the true world-frame acceleration; gravity enters only through qdd
+ * The articulated-body algorithm is affine in f, so acceleration(f + J^T F) = acceleration(f) + inv_inertia F for any F in
+ * R^M.  Inputs: q, qd, f [B, n_dofs], table; device pointers, outputs must not alias inputs.  No allocation, no
+ * synchronisation (graph-capturable).  batch == 0 is a no-op.  DRMB200_EINVAL for n_ee outside [1, 8], a link index out of
+ * range, a link requested twice, a negative batch or a null input; DRMB200_ELIMIT for more live branch points than the
+ * forward-dynamics kernel handles or when a one-row CTA needs more than 227 KB of shared memory.
+ */
+int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links,
+                                       const float* table, const float* q, const float* qd, const float* f,
+                                       int64_t batch, uint32_t flags, int32_t position_only, float* inv_inertia,
+                                       float* acceleration, float* velocity, float* bias_acceleration,
+                                       void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state
