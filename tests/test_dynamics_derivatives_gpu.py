@@ -16,6 +16,7 @@ from differentiable_robot_model_b200.rigid_body_params import UnconstrainedTenso
 from conftest import GOLDEN_DIR, URDFS, urdf_path
 import derivatives_oracle as D
 import synthetic_robots as S
+import tile_mirrors as TM
 from oracle import drm_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -25,7 +26,6 @@ SMALL, LARGE = 131, 4099
 LARGE_ROWS = torch.cat([torch.arange(SMALL, LARGE - 3, 97), torch.arange(LARGE - 3, LARGE)])
 ID_FLAGS = [(True, True), (True, False), (False, True), (False, False)]
 FD_FLAGS = [(True, False), (True, True)]
-SMEM_CAP = 227 * 1024
 
 
 def per_config_error(got, want):
@@ -347,21 +347,6 @@ def test_edge_cases():
 FAM = S.families()
 
 
-def deriv_smem_bytes(n, N, slots, fold_full, fd, static=128):
-    """Shared memory of one CTA of the derivatives kernel: DerivSmemLayout and the tile choice of launch_derivatives."""
-    up4 = lambda x: (x + 3) & ~3  # noqa: E731
-
-    def floats(tc):
-        s = tc * n
-        o = 3 * up4(s) + (3 if fd else 2) * up4(s * n) + N * 28
-        o += up4(max(N * (32 if fd else 20) * s, fold_full * 40))
-        return o + slots * (96 if fd else 36) * s
-    tc = max(1, 128 // n)
-    while tc > 1 and 4 * floats(tc) + static > 113 * 1024:
-        tc -= 1
-    return 4 * floats(tc) + static
-
-
 @pytest.fixture(scope="module")
 def model_dir(tmp_path_factory):
     return str(tmp_path_factory.mktemp("synthetic_deriv"))
@@ -388,30 +373,32 @@ def test_synthetic_families_match_oracle_or_are_refused(name, model_dir):
         assert engine.inverse_dynamics_derivatives_raw(topo, table, z, z, z, 3)[0].shape == (5, 0, 0)
         assert engine.forward_dynamics_derivatives_raw(topo, table, z, z, z, 1)[2].shape == (5, 0, 0)
         return
-    foldable = S.foldable(par, mov)
-    N = 1 + n if foldable else len(par)
-    slots = S.live_slots(S.reduced_parents(par, mov)) if foldable else S.live_slots(par)
     for fd in (False, True):
-        need = deriv_smem_bytes(n, N, slots, len(par) if foldable else 0, fd)
-        call = (lambda: engine.forward_dynamics_derivatives_raw(topo, table, *inp, 1)) if fd else \
-            (lambda: engine.inverse_dynamics_derivatives_raw(topo, table, *inp, 3))
+        # the outcome the host code gives (tests/tile_mirrors.py, pinned to it by tests/test_tile_choice.py)
+        tile, need = TM.deriv_choice(*TM.deriv_program(par, mov), fd)
+        call = (lambda: engine.forward_dynamics_derivatives_raw(topo, table, *inp, flags)) if fd else \
+            (lambda: engine.inverse_dynamics_derivatives_raw(topo, table, *inp, flags))
         q, qd, qdd, f = inputs(r32, LARGE, seed=17)
         for B in (SMALL, LARGE):
             inp = [t[:B].to(DEV) for t in ((q, qd, f) if fd else (q, qd, qdd))]
-            if need > SMEM_CAP:
+            if tile is None:
+                flags = 3
                 before = engine.launch_count()
-                with pytest.raises(RuntimeError, match=r"needs \d+ B of shared memory per CTA"):
+                with pytest.raises(RuntimeError, match=rf"needs {need} B of shared memory per CTA"):
                     call()
                 assert engine.launch_count() == before
                 break
-            got = call()
             rows = oracle_rows(B)
             sub = [t[rows] for t in (q, qd, f if fd else qdd)]
             fn = D.forward_dynamics_derivatives if fd else D.inverse_dynamics_derivatives
-            w64 = fn(r64, *(t.double() for t in sub), True, not fd)
-            w32 = fn(r32, *sub, True, not fd)
-            for k in range(len(got)):
-                check(f"{name} {'FD' if fd else 'ID'} B={B} out{k}", got[k].cpu()[rows], w64[k], w32[k])
+            for grav, damp in ((True, not fd), (True, True)) if fd else ((True, True),):
+                flags = (engine.GRAVITY if grav else 0) | (engine.DAMPING if damp else 0)
+                got = call()
+                w64 = fn(r64, *(t.double() for t in sub), grav, damp)
+                w32 = fn(r32, *sub, grav, damp)
+                for k in range(len(got)):
+                    check(f"{name} {'FD' if fd else 'ID'} TC={tile} B={B} g{grav:d}d{damp:d} out{k}", got[k].cpu()[rows], w64[k],
+                          w32[k])
 
 
 def test_nine_slot_model_is_refused_like_rnea_and_aba(model_dir):

@@ -17,6 +17,7 @@ from conftest import GOLDEN_DIR, URDFS, urdf_path
 import derivatives_oracle as D
 import osd_oracle as S
 import synthetic_robots as SR
+import tile_mirrors as TM
 from oracle import drm_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -395,27 +396,33 @@ def model_dir(tmp_path_factory):
 
 @pytest.mark.parametrize("name", sorted(FAM))
 def test_synthetic_families_match_oracle_or_are_refused(name, model_dir):
-    path = SR.build(FAM[name], model_dir)
+    """Every flag combination, pose and position mode.  The expected outcome is the host code's (tests/tile_mirrors.py,
+    pinned to it by tests/test_tile_choice.py): no family needs more than 227 KB for one row, so none is refused."""
+    spec = FAM[name]
+    path = SR.build(spec, model_dir)
     m = drm.DifferentiableRobotModel(path, name, device=DEV)
     r32, r64, table = robots(path, True)
     names = r32.names
     links = list(dict.fromkeys([names[-1], names[len(names) // 2], names[0]]))
     idx = [r32.index(nm) for nm in links]
+    par, mov = spec.doc()
     q, qd, f = inputs(r32, 37, seed=17)
-    before = engine.launch_count()
-    try:
-        got = engine.operational_space_dynamics_raw(m._topology, idx, table, q.to(DEV), qd.to(DEV), f.to(DEV), engine.GRAVITY)
-    except RuntimeError as e:
-        assert "ELIMIT" in str(e) or "shared memory per CTA" in str(e) or "live branch points" in str(e), str(e)
-        assert engine.launch_count() == before
-        return
-    if r32.n_dofs == 0:
-        for t in got:
-            assert torch.all(t == 0)
-        return
     rows = torch.arange(0, 37, 4)
     sub = [t[rows] for t in (q, qd, f)]
-    w64 = S.operational_space_dynamics(r64, *(t.double() for t in sub), links, True, False)
-    w32 = S.operational_space_dynamics(r32, *sub, links, True, False)
-    for k, nm in enumerate(NAMES):
-        check(f"{name} {nm}", got[k].cpu()[rows], w64[k], w32[k])
+    o64 = OraclePieces(r64, *(t.double() for t in sub), links) if r32.n_dofs else None
+    o32 = OraclePieces(r32, *sub, links) if r32.n_dofs else None
+    for pos in (False, True):
+        tile, need = TM.osd_choice(par, mov, idx, not pos)
+        assert tile is not None, f"{name}: the mirror expects a refusal ({need} B)"
+        for grav, damp in FLAGS:
+            flags = (engine.GRAVITY if grav else 0) | (engine.DAMPING if damp else 0)
+            got = engine.operational_space_dynamics_raw(m._topology, idx, table, q.to(DEV), qd.to(DEV), f.to(DEV), flags,
+                                                        position_only=pos)
+            if r32.n_dofs == 0:
+                for t in got:
+                    assert torch.all(t == 0)
+                continue
+            w64 = o64.outputs(grav, damp, None, pos)
+            w32 = o32.outputs(grav, damp, None, pos)
+            for k, nm in enumerate(NAMES):
+                check(f"{name} T={tile} pos={pos} g{grav:d}d{damp:d} {nm}", got[k].cpu()[rows], w64[k], w32[k])
