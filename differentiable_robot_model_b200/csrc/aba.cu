@@ -29,6 +29,7 @@
 // Algorithmic HBM bytes per configuration: 12n in + 4n out = 16n (112 B at n = 7); at roughly 6 kflop per 7-DoF
 // configuration the kernel is FP32-issue-bound, like RNEA.
 #include "aba_body.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -114,53 +115,29 @@ aba_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ Fol
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <int T>
-static int launch_aba(const TreeProgram& prog, const FoldProgram& fold, const AbaArgs& args, size_t smem_bytes, cudaStream_t stream) {
-    static size_t configured_by_dev[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(aba_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    aba_kernel<T><<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, fold, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("aba launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
-}
-
 static int forward_dynamics_device_impl(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                                        const float* f, int64_t batch, uint32_t flags, float* qdd, cudaStream_t stream,
                                        bool prefolded) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    if (prefolded && !cp->foldable) { set_error("this topology has no link behind a fixed joint to fold"); return DRMB200_EINVAL; }
-    const bool folded = prefolded || (cp->foldable && get_option(11) != 0);      // "rnea_fold"
-    const TreeProgram& prog = folded ? cp->red : cp->full;
-    FoldProgram fold = cp->fold;
-    if (!folded) fold.n_red = 0;
-    if (prefolded) fold.n_full = 0;                     // `table` holds the rows of drmb200_fold_link_table
+    FoldChoice fc;
+    const int rc = select_fold(topo, prefolded, &fc);
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
     if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
     if (batch == 0 || prog.n_dofs == 0) return DRMB200_OK;
     if (table == nullptr || q == nullptr || qd == nullptr || f == nullptr || qdd == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
 
     AbaArgs args;
     args.table = table; args.q = q; args.qd = qd; args.f = f; args.qdd = qdd; args.batch = batch; args.flags = flags;
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd) && al16(f) && al16(qdd)) ? 1 : 0;
+    args.aligned = aligned16(q, qd, f, qdd);
 
     // 64 configurations per CTA unless the model's per-link state would leave a single CTA per SM
-    auto bytes_of = [&](int T) { return (size_t)AbaSmemLayout(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float); };
-    const int tile = bytes_of(64) <= 113 * 1024 ? 64 : 32;
-    const size_t smem_bytes = bytes_of(tile);
-    if (smem_bytes > 227 * 1024) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
-    return tile == 64 ? launch_aba<64>(prog, fold, args, smem_bytes, stream) : launch_aba<32>(prog, fold, args, smem_bytes, stream);
+    const TileChoice c = tile_64_or_32([&](int T) {
+        return (size_t)AbaSmemLayout(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float);
+    });
+    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
+    const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    return c.tile == 64 ? launch_kernel<aba_kernel<64>>(tiles, 64, c.bytes, stream, false, "aba", prog, fc.fold, args)
+                        : launch_kernel<aba_kernel<32>>(tiles, 32, c.bytes, stream, false, "aba", prog, fc.fold, args);
 }
 
 int forward_dynamics_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -219,23 +219,9 @@ int64_t table_grad_workspace_bytes(const drmb200_topology_t* topo, int64_t batch
 int launch_reduce(const float* partials, int grid, const drmb200_topology_t* topo, float* table_grad,
                          cudaStream_t stream) {
     const int entries = topo->n_links * DRMB200_TABLE_STRIDE;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((entries * 32 + 255) / 256);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, reduce_partials_kernel, partials, grid, entries, table_grad);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("reduce launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return launch_kernel<reduce_partials_kernel>((entries * 32 + 255) / 256, 256, 0, stream, true, "reduce", partials, grid, entries,
+                                                 table_grad);
 }
-
 
 int fk_jacobian_backward_device(const drmb200_topology_t* topo, int32_t ee_link, const float* table, const float* q,
                                 int64_t batch, const float* g_pos, const float* g_quat, const float* g_jl,
@@ -253,32 +239,25 @@ int fk_jacobian_backward_device(const drmb200_topology_t* topo, int32_t ee_link,
     args.table = table; args.q = q; args.g_pos = g_pos; args.g_quat = g_quat; args.g_jl = g_jl; args.g_ja = g_ja;
     args.q_grad = q_grad; args.partials = static_cast<float*>(workspace); args.batch = batch;
     args.n_links = topo->n_links;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.vec_ok = (al16(q) && al16(g_pos) && al16(g_quat) && al16(g_jl) && al16(g_ja) && al16(q_grad)) ? 1 : 0;
+    args.vec_ok = aligned16(q, g_pos, g_quat, g_jl, g_ja, q_grad);
 
     int tile = 32, best_warps = 0;           // the tile that keeps the most warps resident per SM
     for (int t = 128; t >= 32; t >>= 1) {
         const size_t b = (size_t)FkBwdSmem(t, prog.n_dofs, prog.len).total_floats * sizeof(float) + 1024;
-        const int warps = b > 227 * 1024 ? 0 : (int)((227 * 1024) / b) * (t / 32);
+        const int warps = b > SMEM_CTA_MAX ? 0 : (int)(SMEM_CTA_MAX / b) * (t / 32);
         if (warps > best_warps) { best_warps = warps; tile = t; }
     }
     const size_t smem_bytes = (size_t)FkBwdSmem(tile, prog.n_dofs, prog.len).total_floats * sizeof(float);
-    if (smem_bytes > 227 * 1024) { set_error("fk backward needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
+    if (smem_bytes > SMEM_CTA_MAX) { set_error("fk backward needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (batch + tile - 1) / tile;
     int grid = 0;
     const bool need_table = table_grad != nullptr;
-#define DRM_LAUNCH_FKB(NT, TT)                                                                                  \
-    do {                                                                                                        \
-        rc = persistent_grid(fk_jacobian_backward_kernel<NT, TT>, TT, smem_bytes, tiles, &grid, "fk backward"); \
-        if (rc != DRMB200_OK) return rc;                                                                        \
-        fk_jacobian_backward_kernel<NT, TT><<<grid, TT, smem_bytes, stream>>>(prog, args);                      \
-    } while (0)
+#define DRM_LAUNCH_FKB(NT, TT) \
+    rc = launch_persistent<fk_jacobian_backward_kernel<NT, TT>>(TT, smem_bytes, tiles, stream, "fk backward", &grid, prog, args)
     if (need_table) { if (tile == 128) DRM_LAUNCH_FKB(true, 128); else if (tile == 64) DRM_LAUNCH_FKB(true, 64); else DRM_LAUNCH_FKB(true, 32); }
     else            { if (tile == 128) DRM_LAUNCH_FKB(false, 128); else if (tile == 64) DRM_LAUNCH_FKB(false, 64); else DRM_LAUNCH_FKB(false, 32); }
 #undef DRM_LAUNCH_FKB
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("fk backward launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
+    if (rc != DRMB200_OK) return rc;
     return need_table ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
 }
 

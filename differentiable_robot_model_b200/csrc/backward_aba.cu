@@ -592,28 +592,21 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     args.scratch = reinterpret_cast<float*>(static_cast<char*>(workspace) + table_grad_workspace_bytes(topo, batch));
     args.batch = batch; args.flags = flags;
     args.accumulate = accumulate_partials ? 1 : 0;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.vec_ok = (al16(q) && al16(qd) && al16(f) && al16(g_qdd) && al16(q_grad) && al16(qd_grad) && al16(f_grad)) ? 1 : 0;
+    args.vec_ok = aligned16(q, qd, f, g_qdd, q_grad, qd_grad, f_grad);
 
     auto bytes_of = [&](int t) { return (size_t)AbaBwdSmem(t, prog.n_dofs, prog.n_links).total_floats * sizeof(float); };
-    const int tile = bytes_of(32) <= 200 * 1024 ? 32 : 16;
+    const int tile = bytes_of(32) <= BWD_SMEM_BUDGET ? 32 : 16;
     const size_t smem_bytes = bytes_of(tile);
-    if (smem_bytes > 227 * 1024) { set_error("forward-dynamics backward needs %zu B of shared memory per CTA (> 227 KB): model too large", smem_bytes); return DRMB200_ELIMIT; }
+    if (smem_bytes > SMEM_CTA_MAX) { set_error("forward-dynamics backward needs %zu B of shared memory per CTA (> 227 KB): model too large", smem_bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (batch + tile - 1) / tile;
     int grid = 0;
     const bool need_table = table_grad != nullptr;
-#define DRM_LAUNCH_ABAB(NT, TT)                                                                                   \
-    do {                                                                                                          \
-        rc = persistent_grid(aba_backward_kernel<NT, TT>, TT < 32 ? 32 : TT, smem_bytes, tiles, &grid, "aba backward"); \
-        if (rc != DRMB200_OK) return rc;                                                                          \
-        aba_backward_kernel<NT, TT><<<grid, TT < 32 ? 32 : TT, smem_bytes, stream>>>(prog, args);                 \
-    } while (0)
+#define DRM_LAUNCH_ABAB(NT, TT) \
+    rc = launch_persistent<aba_backward_kernel<NT, TT>>(TT < 32 ? 32 : TT, smem_bytes, tiles, stream, "aba backward", &grid, prog, args)
     if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB(true, 32); else DRM_LAUNCH_ABAB(true, 16); }
     else            { if (tile == 32) DRM_LAUNCH_ABAB(false, 32); else DRM_LAUNCH_ABAB(false, 16); }
 #undef DRM_LAUNCH_ABAB
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("aba backward launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
+    if (rc != DRMB200_OK) return rc;
     return need_table && reduce ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
 }
 

@@ -1,6 +1,6 @@
 // backward_common.cuh -- helpers shared by the reverse-mode kernels (backward.cu: FK / Jacobian, backward_rnea.cu: RNEA).
 #pragma once
-#include "drm_common.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -96,20 +96,24 @@ __device__ __forceinline__ M3 quat_backward(const M3& R, float4 g) {
 }
 
 
-template <typename Kern>
-static int persistent_grid(Kern kern, int block, size_t smem_bytes, int64_t tiles, int* grid_out, const char* what) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-    if (e != cudaSuccess) { set_error("%s: cudaFuncSetAttribute(%zu B smem): %s", what, smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
+// A persistent kernel: as many CTAs as fit on the device at once (occupancy queried per call, after Kern's
+// dynamic-shared-memory attribute has been raised), at most BWD_MAX_GRID and at most one per tile.  *grid_out: the CTA
+// count, i.e. the number of partial tables the kernel writes.
+template <auto Kern, typename... Args>
+static int launch_persistent(int block, size_t smem_bytes, int64_t tiles, cudaStream_t stream, const char* what, int* grid_out,
+                             const Args&... args) {
+    const int rc = ensure_dynamic_smem<Kern>(smem_bytes);
+    if (rc != DRMB200_OK) return rc;
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, block, smem_bytes);
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, Kern, block, smem_bytes);
     if (e != cudaSuccess || per_sm < 1) { set_error("%s: kernel does not fit on an SM (%zu B smem)", what, smem_bytes); return DRMB200_ECUDA; }
     int64_t grid = (int64_t)sms * per_sm;
     if (grid > BWD_MAX_GRID) grid = BWD_MAX_GRID;
     if (grid > tiles) grid = tiles;
     *grid_out = (int)grid;
-    return DRMB200_OK;
+    return launch_kernel<Kern>(grid, block, smem_bytes, stream, false, what, args...);
 }
 
 

@@ -806,8 +806,7 @@ int inverse_dynamics_backward_device(const drmb200_topology_t* topo, const float
     args.table = table; args.q = q; args.qd = qd; args.qdd = qdd; args.g_tau = g_tau;
     args.q_grad = q_grad; args.qd_grad = qd_grad; args.qdd_grad = qdd_grad;
     args.partials = static_cast<float*>(workspace); args.batch = batch; args.flags = flags;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.vec_ok = (al16(q) && al16(qd) && al16(qdd) && al16(g_tau) && al16(q_grad) && al16(qd_grad) && al16(qdd_grad)) ? 1 : 0;
+    args.vec_ok = aligned16(q, qd, qdd, g_tau, q_grad, qd_grad, qdd_grad);
 
     if ((flags & DRMB200_INERTIAL_GRADS_ONLY) && table_grad != nullptr) {
         if (q_grad != nullptr || qd_grad != nullptr || qdd_grad != nullptr) {
@@ -816,17 +815,16 @@ int inverse_dynamics_backward_device(const drmb200_topology_t* topo, const float
         }
         constexpr int TI = 128;
         const size_t sb = (size_t)RneaInertialSmem(TI, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float);
-        if (sb > 227 * 1024) { set_error("rnea inertial backward needs %zu B of shared memory (> 227 KB)", sb); return DRMB200_ELIMIT; }
+        if (sb > SMEM_CTA_MAX) { set_error("rnea inertial backward needs %zu B of shared memory (> 227 KB)", sb); return DRMB200_ELIMIT; }
         int g = 0;
-        rc = persistent_grid(rnea_backward_inertial_kernel<TI>, TI, sb, (batch + TI - 1) / TI, &g, "rnea inertial backward");
+        rc = launch_persistent<rnea_backward_inertial_kernel<TI>>(TI, sb, (batch + TI - 1) / TI, stream, "rnea inertial backward", &g,
+                                                                  prog, args);
         if (rc != DRMB200_OK) return rc;
-        rnea_backward_inertial_kernel<TI><<<g, TI, sb, stream>>>(prog, args);
-        cudaError_t ei = cudaGetLastError();
-        if (ei != cudaSuccess) { set_error("rnea inertial backward launch: %s", cudaGetErrorString(ei)); return DRMB200_ECUDA; }
-        count_launch();
         return launch_reduce(args.partials, g, topo, table_grad, stream);
     }
 
+    int grid = 0;
+    const bool need_table = table_grad != nullptr;
     // a serial chain (every link's parent is the link before it): the two-sweep kernel
     bool chain = get_option(13) != 0 && prog.n_links >= 2;
     for (int i = 1; i < prog.n_links && chain; ++i) chain = prog.parent[i] == i - 1;
@@ -834,26 +832,18 @@ int inverse_dynamics_backward_device(const drmb200_topology_t* topo, const float
         // 64 rows per CTA: registers allow 7 CTAs (448 configurations) per SM; 128 only when 64 does not fit in shared memory
         int tile = 64;
         size_t sb = (size_t)RneaChainSmem(64, prog.n_dofs, prog.n_links).total_floats * sizeof(float);
-        if (7 * (sb + 1024) > 228 * 1024 && (size_t)RneaChainSmem(32, prog.n_dofs, prog.n_links).total_floats * sizeof(float) <= 227 * 1024) {
+        if (7 * (sb + 1024) > 228 * 1024 && (size_t)RneaChainSmem(32, prog.n_dofs, prog.n_links).total_floats * sizeof(float) <= SMEM_CTA_MAX) {
             tile = 32;
             sb = (size_t)RneaChainSmem(32, prog.n_dofs, prog.n_links).total_floats * sizeof(float);
         }
-        if (sb <= 227 * 1024) {
+        if (sb <= SMEM_CTA_MAX) {
             const int64_t tiles = (batch + tile - 1) / tile;
-            const bool need_table = table_grad != nullptr;
-            int grid = 0;
-#define DRM_LAUNCH_IDC(NT, TT)                                                                                    \
-    do {                                                                                                          \
-        rc = persistent_grid(rnea_backward_chain_kernel<NT, TT>, TT, sb, tiles, &grid, "rnea chain backward");    \
-        if (rc != DRMB200_OK) return rc;                                                                          \
-        rnea_backward_chain_kernel<NT, TT><<<grid, TT, sb, stream>>>(prog, args);                                 \
-    } while (0)
+#define DRM_LAUNCH_IDC(NT, TT) \
+    rc = launch_persistent<rnea_backward_chain_kernel<NT, TT>>(TT, sb, tiles, stream, "rnea chain backward", &grid, prog, args)
             if (need_table) { if (tile == 64) DRM_LAUNCH_IDC(true, 64); else DRM_LAUNCH_IDC(true, 32); }
             else            { if (tile == 64) DRM_LAUNCH_IDC(false, 64); else DRM_LAUNCH_IDC(false, 32); }
 #undef DRM_LAUNCH_IDC
-            cudaError_t ec = cudaGetLastError();
-            if (ec != cudaSuccess) { set_error("rnea chain backward launch: %s", cudaGetErrorString(ec)); return DRMB200_ECUDA; }
-            count_launch();
+            if (rc != DRMB200_OK) return rc;
             return need_table ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
         }
     }
@@ -863,26 +853,18 @@ int inverse_dynamics_backward_device(const drmb200_topology_t* topo, const float
     int tile = 32, best_warps = 0;
     for (int t = 128; t >= 32; t >>= 1) {
         const size_t b = (size_t)RneaBwdSmem(t, prog.n_dofs, prog.n_links, prog.n_slots, prog.n_tips).total_floats * sizeof(float) + 1024;
-        const int warps = b > 227 * 1024 ? 0 : (int)((227 * 1024) / b) * (t / 32);
+        const int warps = b > SMEM_CTA_MAX ? 0 : (int)(SMEM_CTA_MAX / b) * (t / 32);
         if (warps > best_warps) { best_warps = warps; tile = t; }
     }
     const size_t smem_bytes = (size_t)RneaBwdSmem(tile, prog.n_dofs, prog.n_links, prog.n_slots, prog.n_tips).total_floats * sizeof(float);
-    if (smem_bytes > 227 * 1024) { set_error("rnea backward needs %zu B of shared memory per CTA (> 227 KB): model too large", smem_bytes); return DRMB200_ELIMIT; }
+    if (smem_bytes > SMEM_CTA_MAX) { set_error("rnea backward needs %zu B of shared memory per CTA (> 227 KB): model too large", smem_bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (batch + tile - 1) / tile;
-    int grid = 0;
-    const bool need_table = table_grad != nullptr;
-#define DRM_LAUNCH_IDB(NT, TT)                                                                              \
-    do {                                                                                                    \
-        rc = persistent_grid(rnea_backward_kernel<NT, TT>, TT, smem_bytes, tiles, &grid, "rnea backward");  \
-        if (rc != DRMB200_OK) return rc;                                                                    \
-        rnea_backward_kernel<NT, TT><<<grid, TT, smem_bytes, stream>>>(prog, args);                         \
-    } while (0)
+#define DRM_LAUNCH_IDB(NT, TT) \
+    rc = launch_persistent<rnea_backward_kernel<NT, TT>>(TT, smem_bytes, tiles, stream, "rnea backward", &grid, prog, args)
     if (need_table) { if (tile == 128) DRM_LAUNCH_IDB(true, 128); else if (tile == 64) DRM_LAUNCH_IDB(true, 64); else DRM_LAUNCH_IDB(true, 32); }
     else            { if (tile == 128) DRM_LAUNCH_IDB(false, 128); else if (tile == 64) DRM_LAUNCH_IDB(false, 64); else DRM_LAUNCH_IDB(false, 32); }
 #undef DRM_LAUNCH_IDB
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("rnea backward launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
+    if (rc != DRMB200_OK) return rc;
     return need_table ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
 }
 

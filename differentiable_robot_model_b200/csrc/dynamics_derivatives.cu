@@ -27,6 +27,7 @@
 // Algorithmic HBM bytes per configuration: 12n in, 8n^2 (ID) / 12n^2 (FD) out.  Every thread repeats its configuration's
 // primal recursion (n times per configuration): the arithmetic, not the bytes, bounds the kernel.
 #include "aba_tangent.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -261,72 +262,45 @@ __global__ void dynamics_derivatives_kernel(const __grid_constant__ TreeProgram 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <bool FD>
-static int launch_derivatives(const TreeProgram& prog, const FoldProgram& fold, DerivArgs args, cudaStream_t stream) {
-    auto kern = dynamics_derivatives_kernel<FD>;
+// ~128 threads per CTA: TC = 128 / n configurations, fewer while the footprint would leave a single CTA per SM.  fold_full:
+// the full link count when the kernel folds the table while staging it (folding scratch), else 0.
+static TileChoice deriv_tile(const TreeProgram& prog, int fold_full, bool fd, size_t static_bytes) {
     const int n = prog.n_dofs;
-    const bool staging_fold = fold.n_red > 0 && fold.n_full > 0;
-    auto bytes_of = [&](int tc) {
-        return (size_t)DerivSmemLayout(tc, n, prog.n_links, prog.n_slots, staging_fold ? fold.n_full : 0, FD).total_floats * sizeof(float);
-    };
-    static cudaFuncAttributes attr_by_dev[64];
-    static size_t configured_by_dev[64] = {0};
-    static bool queried_by_dev[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!queried_by_dev[dev & 63]) {
-        cudaError_t e = cudaFuncGetAttributes(&attr_by_dev[dev & 63], kern);
-        if (e != cudaSuccess) { set_error("cudaFuncGetAttributes: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        queried_by_dev[dev & 63] = true;
-    }
-    const size_t static_bytes = attr_by_dev[dev & 63].sharedSizeBytes;
-    // ~128 threads per CTA, fewer configurations while the footprint would leave a single CTA per SM
-    int tc = n >= 128 ? 1 : 128 / n;
-    while (tc > 1 && bytes_of(tc) + static_bytes > 113 * 1024) --tc;
-    const size_t smem_bytes = bytes_of(tc);
-    if (smem_bytes + static_bytes > 227 * 1024) {
-        set_error("model needs %zu B of shared memory per CTA (> 227 KB) for its %s derivatives", smem_bytes + static_bytes,
-                  FD ? "forward-dynamics" : "inverse-dynamics");
-        return DRMB200_ELIMIT;
-    }
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + tc - 1) / tc;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    args.tc = tc;
-    kern<<<(unsigned)tiles, tc * n, smem_bytes, stream>>>(prog, fold, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("dynamics derivatives launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return tile_count_down(n >= 128 ? 1 : 128 / n, [&](int tc) {
+        return (size_t)DerivSmemLayout(tc, n, prog.n_links, prog.n_slots, fold_full, fd).total_floats * sizeof(float);
+    }, static_bytes);
 }
 
 template <bool FD>
 static int derivatives_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd, const float* x3,
                               int64_t batch, uint32_t flags, float* o0, float* o1, float* o2, cudaStream_t stream, bool prefolded) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    if (prefolded && !cp->foldable) { set_error("this topology has no link behind a fixed joint to fold"); return DRMB200_EINVAL; }
-    const bool folded = prefolded || (cp->foldable && get_option(11) != 0);      // "rnea_fold"
-    const TreeProgram& prog = folded ? cp->red : cp->full;
-    FoldProgram fold = cp->fold;
-    if (!folded) fold.n_red = 0;                        // the kernel's "no folding" flag
-    if (prefolded) fold.n_full = 0;                     // ... and its "rows are folded already" flag
+    FoldChoice fc;
+    int rc = select_fold(topo, prefolded, &fc);
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
     if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
     if (batch == 0 || prog.n_dofs == 0 || (o0 == nullptr && o1 == nullptr && o2 == nullptr)) return DRMB200_OK;
     if (table == nullptr || q == nullptr || qd == nullptr || x3 == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
     DerivArgs args;
     args.table = table; args.q = q; args.qd = qd; args.x3 = x3;
     args.out[0] = o0; args.out[1] = o1; args.out[2] = o2;
-    args.batch = batch; args.flags = flags & (DRMB200_GRAVITY | DRMB200_DAMPING); args.tc = 0;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd) && al16(x3) && al16(o0) && al16(o1) && al16(o2)) ? 1 : 0;
-    return launch_derivatives<FD>(prog, fold, args, stream);
+    args.batch = batch; args.flags = flags & (DRMB200_GRAVITY | DRMB200_DAMPING);
+    args.aligned = aligned16(q, qd, x3, o0, o1, o2);
+
+    constexpr auto kern = dynamics_derivatives_kernel<FD>;
+    size_t static_bytes;
+    rc = static_smem_bytes<kern>(&static_bytes);
+    if (rc != DRMB200_OK) return rc;
+    const bool staging_fold = fc.fold.n_red > 0 && fc.fold.n_full > 0;
+    const TileChoice c = deriv_tile(prog, staging_fold ? fc.fold.n_full : 0, FD, static_bytes);
+    if (c.bytes + static_bytes > SMEM_CTA_MAX) {
+        set_error("model needs %zu B of shared memory per CTA (> 227 KB) for its %s derivatives", c.bytes + static_bytes,
+                  FD ? "forward-dynamics" : "inverse-dynamics");
+        return DRMB200_ELIMIT;
+    }
+    args.tc = c.tile;
+    return launch_kernel<kern>((batch + c.tile - 1) / c.tile, c.tile * prog.n_dofs, c.bytes, stream, false, "dynamics derivatives", prog,
+                               fc.fold, args);
 }
 
 int inverse_dynamics_derivatives_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -28,7 +28,7 @@
 // (224 B for the 7-DoF Kuka iiwa) -- SURVEY.md section 8(d).
 #include <cstring>
 #include <mutex>
-#include "drm_common.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -460,40 +460,16 @@ int build_path_program(const drmb200_topology_t* topo, int32_t ee_link, PathProg
 
 template <int NDOF, int TILE, bool WITH_JAC, int MAXLEN>
 static int launch_fk(const PathProgram& prog, const FkArgs& args, cudaStream_t stream) {
-    const FkSmemLayout L(TILE, prog.n_dofs, prog.len, WITH_JAC);
-    const size_t smem_bytes = (size_t)L.total_floats * sizeof(float);
-    auto kern = fk_jacobian_kernel<NDOF, TILE, WITH_JAC, MAXLEN>;
-    cudaFuncAttributes fa;
-    const size_t static_bytes = cudaFuncGetAttributes(&fa, kern) == cudaSuccess ? fa.sharedSizeBytes : 1024;
-    if (smem_bytes + static_bytes > 227 * 1024) {
+    constexpr auto kern = fk_jacobian_kernel<NDOF, TILE, WITH_JAC, MAXLEN>;
+    const size_t smem_bytes = (size_t)FkSmemLayout(TILE, prog.n_dofs, prog.len, WITH_JAC).total_floats * sizeof(float);
+    size_t static_bytes;
+    const int rc = static_smem_bytes<kern>(&static_bytes);
+    if (rc != DRMB200_OK) return rc;
+    if (smem_bytes + static_bytes > SMEM_CTA_MAX) {
         set_error("fk kernel needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes + static_bytes);
         return DRMB200_ELIMIT;
     }
-    static size_t configured_by_dev[64] = {0};     // per instantiation, per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + TILE - 1) / TILE;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)tiles);
-    cfg.blockDim = dim3(TILE);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = args.pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, prog, args);
-    if (e != cudaSuccess) { set_error("fk_jacobian launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return launch_kernel<kern>((args.batch + TILE - 1) / TILE, TILE, smem_bytes, stream, args.pdl != 0, "fk_jacobian", prog, args);
 }
 
 template <int NDOF, int TILE, bool WITH_JAC>
@@ -620,8 +596,7 @@ int fk_jacobian_device(const drmb200_topology_t* topo, int32_t ee_link, const fl
     FkArgs args;
     args.table = table; args.q = q; args.pos = pos; args.quat = quat; args.jlin = jlin; args.jang = jang;
     args.batch = batch;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(pos) && al16(quat) && al16(jlin) && al16(jang)) ? 1 : 0;
+    args.aligned = aligned16(q, pos, quat, jlin, jang);
     args.use_bulk = get_option(0) != 0;
     const bool with_jac = jlin != nullptr;
     // n_dofs % 4 == 0 (Allegro, n = 16): the per-lane rows of this kernel's natural-layout tiles are 16-way bank
@@ -645,7 +620,7 @@ int fk_jacobian_device(const drmb200_topology_t* topo, int32_t ee_link, const fl
         tile = (prog.n_dofs > 8 || (batch <= (int64_t)device_sm_count() * 1024 && args.pdl != 2)) ? 128 : 64;
     // a long path with many Jacobian columns (e.g. a 63-DoF chain) does not fit 128 rows: take 64 (the kernel's static
     // shared memory counts against the same 227 KB, hence the margin)
-    if (tile == 128 && (size_t)FkSmemLayout(128, prog.n_dofs, prog.len, with_jac).total_floats * sizeof(float) + 1024 > 227 * 1024)
+    if (tile == 128 && (size_t)FkSmemLayout(128, prog.n_dofs, prog.len, with_jac).total_floats * sizeof(float) + 1024 > SMEM_CTA_MAX)
         tile = 64;
     switch (prog.n_dofs) {
         case 2: return launch_fk_t<2>(tile, with_jac, prog, args, stream);

@@ -24,6 +24,7 @@
 // Outputs are [n_ee, B, ...] blocks.  Algorithmic HBM bytes per configuration: 4n + n_ee (28 + 24n)  (Allegro, 4 tips:
 // 64 + 4 * 412 = 1712 B, SURVEY.md section 8d).
 #include <cstring>
+#include "launch.cuh"
 #include "multi_program.cuh"
 
 namespace drm {
@@ -402,12 +403,22 @@ int build_multi_program(const drmb200_topology_t* topo, int32_t n_ee, const int3
     return DRMB200_OK;
 }
 
+int build_union_program(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, UnionProgram* prog) {
+    const int rc = build_multi_program(topo, n_ee, ee_links, &prog->walk);
+    if (rc != DRMB200_OK) return rc;
+    const MultiProgram& W = prog->walk;
+    prog->n_u = 0;
+    for (int k = 0; k < W.n_steps; ++k)
+        if (W.dof[k] >= 0) prog->u_dof[prog->n_u++] = W.dof[k];
+    return DRMB200_OK;
+}
+
 template <int NDOF, bool CHUNK, bool WITH_JAC>
 static int launch_fk_tree(const MultiProgram& prog, const MtArgs& args, cudaStream_t stream) {
     const MtWarpLayout L(prog.n_dofs, prog.n_jslots, prog.n_state_slots, WITH_JAC, args.nbuf);
     const size_t warp_bytes = (size_t)L.warp_floats * sizeof(float);
     const size_t tab_bytes = (size_t)mt_table_floats(prog.n_steps) * sizeof(float);
-    const size_t cap = 227 * 1024 - 256;
+    const size_t cap = SMEM_CTA_MAX - 256;
     if (tab_bytes + warp_bytes > cap) { set_error("multi-ee FK needs %zu B of shared memory per warp (> 227 KB)", tab_bytes + warp_bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (args.batch + 31) >> 5;
     const int sms = device_sm_count();
@@ -423,16 +434,6 @@ static int launch_fk_tree(const MultiProgram& prog, const MtArgs& args, cudaStre
     if (grid_cap > 0 && grid_cap < per_sm) per_sm = grid_cap;
     int64_t ctas = (tiles + warps - 1) / warps;
     if (ctas > (int64_t)sms * per_sm) ctas = (int64_t)sms * per_sm;
-    auto kern = fk_tree_kernel<NDOF, CHUNK, WITH_JAC>;
-    static size_t configured_by_dev[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
     MtArgs largs = args;
     if (args.pdl < 0) {                                   // decide: hazards against the FK launches in flight, residency share
         const uintptr_t Bn = (uintptr_t)args.batch * (uintptr_t)prog.n_ee, n = (uintptr_t)prog.n_dofs;
@@ -443,20 +444,8 @@ static int launch_fk_tree(const MultiProgram& prog, const MtArgs& args, cudaStre
         const int mode = pdl_decide(stream, ins, 2, outs, (double)ctas * (double)smem_bytes);
         largs.pdl = mode == 2 ? 2 : 0;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)ctas);
-    cfg.blockDim = dim3(32u * warps);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = largs.pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, prog, largs);
-    if (e != cudaSuccess) { set_error("fk_tree launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return launch_kernel<fk_tree_kernel<NDOF, CHUNK, WITH_JAC>>(ctas, 32 * warps, smem_bytes, stream, largs.pdl != 0, "fk_tree", prog,
+                                                              largs);
 }
 template <int NDOF, bool CHUNK>
 static int launch_fk_tree_j(bool with_jac, const MultiProgram& prog, const MtArgs& args, cudaStream_t stream) {
@@ -491,9 +480,8 @@ int fk_jacobian_multi_device(const drmb200_topology_t* topo, int32_t n_ee, const
     if (pos == nullptr && quat == nullptr && jlin == nullptr) return DRMB200_OK;
     MtArgs args;
     args.table = table; args.q = q; args.pos = pos; args.quat = quat; args.jlin = jlin; args.jang = jang; args.batch = batch;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
     // every [e] block must start 16-byte aligned too: B * 12 bytes (pos) is a multiple of 16 only when B % 4 == 0
-    args.aligned = (al16(q) && al16(pos) && al16(quat) && al16(jlin) && al16(jang) && (n_ee == 1 || (batch & 3) == 0)) ? 1 : 0;
+    args.aligned = aligned16(q, pos, quat, jlin, jang) && (n_ee == 1 || (batch & 3) == 0);
     args.use_bulk = get_option(0) != 0;
     args.nbuf = get_option(10) == 2 ? 2 : 1;
     args.pdl = -1;                                        // decided at launch (pdl_decide)

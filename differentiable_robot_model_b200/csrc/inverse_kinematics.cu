@@ -21,13 +21,10 @@
 // A, its Cholesky factor, e and y stay in registers.  HBM traffic per row is 4n + 28 B in and 4n + 13 B out, independent
 // of max_iters: the kernel is arithmetic-bound.
 #include <cmath>
-#include "drm_common.cuh"
+#include "ik_common.cuh"
+#include "launch.cuh"
 
 namespace drm {
-
-// compiled-in constants (include/drm_b200.h documents them; DESIGN.md §3 records the evidence behind them)
-constexpr float IK_LAMBDA_MIN = 1e-5f;
-constexpr float IK_LAMBDA_MAX = 1e5f;
 
 struct IkArgs {
     const float* __restrict__ table;       // [n_links, 28]
@@ -60,10 +57,6 @@ struct IkSmemLayout {
         total_floats = o;
     }
 };
-
-__device__ __forceinline__ float clamp_joint(float x, const float* s_lim, int n, int c, bool limits) {
-    return limits ? fminf(fmaxf(x, s_lim[c]), s_lim[n + c]) : x;
-}
 
 // Pose and error of one configuration.  qx: this row's q slots (stride T); J: this row's Jacobian slots, rows 0..2 J_lin,
 // 3..5 J_ang (only path columns are written; the others stay zero).  Returns E; e[0..M) and the two error norms.
@@ -104,19 +97,7 @@ __device__ __forceinline__ float evaluate(const PathProgram& prog, const float* 
     perr = sqrtf(E);
     rerr = 0.f;
     if (POSE) {
-        if (prog.ee_axis != 0) R = unpermute_cols(R, prog.ee_axis);
-        const float4 c = quat_xyzw(R);
-        const float ax = tgt[3 * T], ay = tgt[4 * T], az = tgt[5 * T], aw = tgt[6 * T];
-        // q_err = quat* (x) conj(quat(R)), Hamilton product, xyzw
-        float w = fmaf(aw, c.w, fmaf(ax, c.x, fmaf(ay, c.y, az * c.z)));
-        float x = fmaf(-aw, c.x, fmaf(ax, c.w, fmaf(-ay, c.z, az * c.y)));
-        float y = fmaf(-aw, c.y, fmaf(ax, c.z, fmaf(ay, c.w, -az * c.x)));
-        float zz = fmaf(-aw, c.z, fmaf(-ax, c.y, fmaf(ay, c.x, az * c.w)));
-        if (w < 0.f) { w = -w; x = -x; y = -y; zz = -zz; }
-        const float s = sqrtf(fmaf(x, x, fmaf(y, y, zz * zz)));
-        const float g = s > 0.f ? 2.f * atan2f(s, w) / s : 0.f;
-        e[3] = g * x; e[4] = g * y; e[5] = g * zz;
-        const float E_rot = fmaf(e[3], e[3], fmaf(e[4], e[4], e[5] * e[5]));
+        const float E_rot = rotvec_error(R, prog.ee_axis, tgt + 3 * T, T, e[3], e[4], e[5]);
         rerr = sqrtf(E_rot);
         E += E_rot;
     }
@@ -139,11 +120,7 @@ inverse_kinematics_kernel(const __grid_constant__ PathProgram prog, const IkArgs
     const bool limits = args.lower != nullptr;
 
     // ---- stage: path rows (signed gather), limits, clamped q0 and the targets, all slot-major -------------------------
-    for (int i = tid; i < prog.len * 12; i += T) {
-        const uint32_t mp = prog.tab_map[i];
-        const float v = __ldg(args.table + (mp & 0x7fffu));
-        s_tab[i] = (mp & 0x8000u) ? -v : v;
-    }
+    stage_walked_rows(s_tab, args.table, prog.tab_map, prog.len * 12, T);
     if (limits)
         for (int c = tid; c < n; c += T) { s_lim[c] = __ldg(args.lower + c); s_lim[n + c] = __ldg(args.upper + c); }
     if (!prog.full_cover)                        // Jacobian columns of joints off the path stay zero in both buffers
@@ -169,11 +146,7 @@ inverse_kinematics_kernel(const __grid_constant__ PathProgram prog, const IkArgs
     if (tid < valid) {
         const int64_t row = tile_start + tid;
         const float* tgt = s_tgt + tid;
-        if (POSE) {                              // the target quaternion, normalised once
-            float* tq = s_tgt + 3 * T + tid;
-            const float inv = 1.f / sqrtf(fmaf(tq[0], tq[0], fmaf(tq[T], tq[T], fmaf(tq[2 * T], tq[2 * T], tq[3 * T] * tq[3 * T]))));
-            tq[0] *= inv; tq[T] *= inv; tq[2 * T] *= inv; tq[3 * T] *= inv;
-        }
+        if (POSE) normalize_target_quat(s_tgt + 3 * T + tid, T);      // the target quaternion, normalised once
         const int nT = n * T;
         float* const q_rows = smem + L.q + tid;             // buffer b of this row: q_rows + b nT, j_rows + 6 b nT
         float* const j_rows = smem + L.jac + tid;
@@ -286,42 +259,25 @@ inverse_kinematics_kernel(const __grid_constant__ PathProgram prog, const IkArgs
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+// 64 rows while two CTAs still fit an SM, else 32 (a 63-DoF chain: ~117 KB at 32 rows)
+static TileChoice ik_tile(const PathProgram& prog, size_t static_bytes) {
+    return tile_64_or_32([&](int T) { return (size_t)IkSmemLayout(T, prog.n_dofs, prog.len).total_floats * sizeof(float); },
+                         static_bytes);
+}
+
 template <bool POSE>
 static int launch_ik(const PathProgram& prog, const IkArgs& args, cudaStream_t stream) {
-    auto kern = inverse_kinematics_kernel<POSE>;
-    static cudaFuncAttributes attr_by_dev[64];
-    static size_t configured_by_dev[64] = {0};
-    static bool queried_by_dev[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!queried_by_dev[dev & 63]) {
-        cudaError_t e = cudaFuncGetAttributes(&attr_by_dev[dev & 63], kern);
-        if (e != cudaSuccess) { set_error("cudaFuncGetAttributes: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        queried_by_dev[dev & 63] = true;
-    }
-    const size_t static_bytes = attr_by_dev[dev & 63].sharedSizeBytes;
-    auto bytes_of = [&](int T) { return (size_t)IkSmemLayout(T, prog.n_dofs, prog.len).total_floats * sizeof(float); };
-    // 64 rows while two CTAs still fit an SM, else 32 (a 63-DoF chain: ~117 KB at 32 rows)
-    const int T = bytes_of(64) + static_bytes <= 113 * 1024 ? 64 : 32;
-    const size_t smem_bytes = bytes_of(T);
-    if (smem_bytes + static_bytes > 227 * 1024) {
-        set_error("inverse kinematics needs %zu B of shared memory per CTA (> 227 KB) for %d joints", smem_bytes + static_bytes,
+    constexpr auto kern = inverse_kinematics_kernel<POSE>;
+    size_t static_bytes;
+    const int rc = static_smem_bytes<kern>(&static_bytes);
+    if (rc != DRMB200_OK) return rc;
+    const TileChoice c = ik_tile(prog, static_bytes);
+    if (c.bytes + static_bytes > SMEM_CTA_MAX) {
+        set_error("inverse kinematics needs %zu B of shared memory per CTA (> 227 KB) for %d joints", c.bytes + static_bytes,
                   prog.n_dofs);
         return DRMB200_ELIMIT;
     }
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    kern<<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("inverse kinematics launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return launch_kernel<kern>((args.batch + c.tile - 1) / c.tile, c.tile, c.bytes, stream, false, "inverse kinematics", prog, args);
 }
 
 int inverse_kinematics_device(const drmb200_topology_t* topo, int32_t ee_link, const float* table, const float* q0,
@@ -336,17 +292,9 @@ int inverse_kinematics_device(const drmb200_topology_t* topo, int32_t ee_link, c
     int movable = 0;
     for (int k = 0; k < prog.len; ++k) movable += prog.dof[k] >= 0;
     if (movable == 0) { set_error("ee_link=%d: no movable joint between the root and this link", ee_link); return DRMB200_EINVAL; }
-    if (max_iters < 0) { set_error("max_iters=%d < 0", max_iters); return DRMB200_EINVAL; }
-    if (!(pos_tol >= 0.f) || !(rot_tol >= 0.f)) { set_error("tolerances must be >= 0 (pos_tol=%g, rot_tol=%g)", pos_tol, rot_tol); return DRMB200_EINVAL; }
-    if ((lower == nullptr) != (upper == nullptr)) { set_error("lower and upper must both be given or both be null"); return DRMB200_EINVAL; }
-    if (!(damping_init > 0.f)) { set_error("damping_init=%g must be > 0", damping_init); return DRMB200_EINVAL; }
-    if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
-    if (batch == 0) return DRMB200_OK;
-    if (table == nullptr || q0 == nullptr || target_pos == nullptr || q == nullptr || pos_err == nullptr || rot_err == nullptr ||
-        converged == nullptr || damping_out == nullptr) {
-        set_error("null pointer argument");
-        return DRMB200_EINVAL;
-    }
+    const int arg_rc = check_ik_arguments(table, q0, target_pos, lower, upper, batch, max_iters, damping_init, pos_tol, rot_tol, q,
+                                          pos_err, rot_err, converged, damping_out);
+    if (arg_rc != DRMB200_OK || batch == 0) return arg_rc;
     IkArgs args;
     args.table = table; args.q0 = q0; args.tpos = target_pos; args.tquat = target_quat;
     args.lower = lower; args.upper = upper; args.damping_in = damping_in;

@@ -27,19 +27,11 @@
 // A no longer fits in registers (the single-link kernel keeps its 6 x 6 there).  HBM traffic per row is independent of
 // max_iters: the kernel is arithmetic-bound.
 #include <cmath>
+#include "ik_common.cuh"
+#include "launch.cuh"
 #include "multi_program.cuh"
 
 namespace drm {
-
-// the single-link kernel's constants (inverse_kinematics.cu), repeated: both are part of the documented algorithm
-constexpr float IKM_LAMBDA_MIN = 1e-5f;
-constexpr float IKM_LAMBDA_MAX = 1e5f;
-
-struct IkmProgram {
-    MultiProgram walk;
-    int32_t n_u;                           // movable joints on the union of the paths
-    int8_t u_dof[DRMB200_MAX_LINKS];       // U column -> q / dof column, in walk order
-};
 
 struct IkmArgs {
     const float* __restrict__ table;       // [n_links, 28]
@@ -81,23 +73,18 @@ struct IkmSmemLayout {
     }
 };
 
-__device__ __forceinline__ float clamp_joint_m(float x, const float* s_lim, int n, int c, bool limits) {
-    return limits ? fminf(fmaxf(x, s_lim[c]), s_lim[n + c]) : x;
-}
 __device__ __forceinline__ int tri(int i, int j) { return i * (i + 1) / 2 + j; }
 
 // Pose errors and stacked Jacobian of one configuration.  qx: this row's q slots; J: this row's J[M][n_u] slots; e: its
 // e[M] slots; jscr / st: its joint scratch and branch-state slots; tgt: its targets (tw slots per link).  Returns E and
 // whether every link is within tolerance.
 template <bool POSE>
-__device__ __forceinline__ float evaluate_multi(const IkmProgram& P, const float* s_tab, const float* qx, float* J, float* e,
+__device__ __forceinline__ float evaluate_multi(const UnionProgram& P, const float* s_tab, const float* qx, float* J, float* e,
                                                 float* jscr, float* st, const float* tgt, int T, float pos_tol, float rot_tol,
                                                 bool& within) {
     constexpr int MR = POSE ? 6 : 3;             // rows per link
     constexpr int TW = POSE ? 7 : 3;
     const MultiProgram& W = P.walk;
-    const int n_u = P.n_u;
-    const int rs = n_u * T;                      // stride between rows of J
     M3 R = identity3();
     V3 p = v3(0.f, 0.f, 0.f);
     float E = 0.f;
@@ -131,18 +118,8 @@ __device__ __forceinline__ float evaluate_multi(const IkmProgram& P, const float
         }
         const int l = W.ee[k];
         if (l < 0) continue;
-        // link l: its rows of J (J_lin = z x p_ee - z x p_i over J_ang = z) and of e
-        float* Jl = J + MR * l * rs;
-        for (int u = 0; u < n_u; ++u) {
-            const int s = W.cslot[l][P.u_dof[u]];
-            if (s < 0) continue;                 // off this link's path: stays zero
-            const float* js = jscr + s * 6 * T;
-            const V3 z = ldv(js, T), m = ldv(js + 3 * T, T);
-            const V3 j = cross_add(z, p, v3(-m.x, -m.y, -m.z));
-            float* col = Jl + u * T;
-            col[0] = j.x; col[rs] = j.y; col[2 * rs] = j.z;
-            if (POSE) { col[3 * rs] = z.x; col[4 * rs] = z.y; col[5 * rs] = z.z; }
-        }
+        // link l: its rows of J and of e
+        link_jacobian(P, l, MR, p, jscr, J, T);
         const float* tl = tgt + TW * l * T;
         float* el = e + MR * l * T;
         const float ex = tl[0] - p.x, ey = tl[T] - p.y, ez = tl[2 * T] - p.z;
@@ -151,21 +128,9 @@ __device__ __forceinline__ float evaluate_multi(const IkmProgram& P, const float
         const float perr = sqrtf(El);
         float rerr = 0.f;
         if (POSE) {
-            M3 Rl = R;
-            if (W.axis[k] != 0) Rl = unpermute_cols(Rl, W.axis[k]);
-            const float4 c4 = quat_xyzw(Rl);
-            const float ax = tl[3 * T], ay = tl[4 * T], az = tl[5 * T], aw = tl[6 * T];
-            // q_err = quat* (x) conj(quat(R)), Hamilton product, xyzw
-            float w = fmaf(aw, c4.w, fmaf(ax, c4.x, fmaf(ay, c4.y, az * c4.z)));
-            float x = fmaf(-aw, c4.x, fmaf(ax, c4.w, fmaf(-ay, c4.z, az * c4.y)));
-            float y = fmaf(-aw, c4.y, fmaf(ax, c4.z, fmaf(ay, c4.w, -az * c4.x)));
-            float zz = fmaf(-aw, c4.z, fmaf(-ax, c4.y, fmaf(ay, c4.x, az * c4.w)));
-            if (w < 0.f) { w = -w; x = -x; y = -y; zz = -zz; }
-            const float s = sqrtf(fmaf(x, x, fmaf(y, y, zz * zz)));
-            const float g = s > 0.f ? 2.f * atan2f(s, w) / s : 0.f;
-            const float rx = g * x, ry = g * y, rz = g * zz;
+            float rx, ry, rz;
+            const float E_rot = rotvec_error(R, W.axis[k], tl + 3 * T, T, rx, ry, rz);
             el[3 * T] = rx; el[4 * T] = ry; el[5 * T] = rz;
-            const float E_rot = fmaf(rx, rx, fmaf(ry, ry, rz * rz));
             rerr = sqrtf(E_rot);
             El += E_rot;
         }
@@ -177,7 +142,7 @@ __device__ __forceinline__ float evaluate_multi(const IkmProgram& P, const float
 
 template <bool POSE>
 __global__ void __launch_bounds__(64)
-inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmArgs args) {
+inverse_kinematics_multi_kernel(const __grid_constant__ UnionProgram P, const IkmArgs args) {
     constexpr int MR = POSE ? 6 : 3;
     extern __shared__ __align__(128) float smem[];
     const MultiProgram& W = P.walk;
@@ -194,11 +159,7 @@ inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmA
     const bool limits = args.lower != nullptr;
 
     // ---- stage: walked rows (signed gather), limits, zeroed Jacobians, clamped q0 and the targets, slot-major ----------
-    for (int i = tid; i < W.n_steps * 12; i += T) {
-        const uint32_t mp = W.tab_map[i];
-        const float v = __ldg(args.table + (mp & 0x7fffu));
-        s_tab[i] = (mp & 0x8000u) ? -v : v;
-    }
+    stage_walked_rows(s_tab, args.table, W.tab_map, W.n_steps * 12, T);
     if (limits)
         for (int c = tid; c < n; c += T) { s_lim[c] = __ldg(args.lower + c); s_lim[n + c] = __ldg(args.upper + c); }
     for (int i = tid; i < 2 * M * n_u * T; i += T) smem[L.jac + i] = 0.f;
@@ -206,7 +167,7 @@ inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmA
     float* s_q = smem + L.q;
     for (int i = tid; i < valid * n; i += T) {   // coalesced global reads; q0 row-major -> slot-major
         const int r = i / n, c = i - r * n;
-        s_q[c * T + r] = clamp_joint_m(__ldg(args.q0 + tile_start * n + i), s_lim, n, c, limits);
+        s_q[c * T + r] = clamp_joint(__ldg(args.q0 + tile_start * n + i), s_lim, n, c, limits);
     }
     float* s_tgt = smem + L.tgt;
     for (int l = 0; l < n_ee; ++l) {
@@ -226,11 +187,7 @@ inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmA
         const int64_t row = tile_start + tid;
         const float* tgt = s_tgt + tid;
         if (POSE)                                // the target quaternions, normalised once
-            for (int l = 0; l < n_ee; ++l) {
-                float* tq = s_tgt + (TW * l + 3) * T + tid;
-                const float inv = 1.f / sqrtf(fmaf(tq[0], tq[0], fmaf(tq[T], tq[T], fmaf(tq[2 * T], tq[2 * T], tq[3 * T] * tq[3 * T]))));
-                tq[0] *= inv; tq[T] *= inv; tq[2 * T] *= inv; tq[3 * T] *= inv;
-            }
+            for (int l = 0; l < n_ee; ++l) normalize_target_quat(s_tgt + (TW * l + 3) * T + tid, T);
         const int nT = n * T, JT = M * n_u * T, rs = n_u * T;
         float* const q_rows = smem + L.q + tid;              // buffer b of this row: q_rows + b nT, j_rows + b JT, e_rows + b M T
         float* const j_rows = smem + L.jac + tid;
@@ -287,7 +244,7 @@ inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmA
                     }
                 }
                 ++it;
-                if (!ok) { lam = fminf(4.f * lam, IKM_LAMBDA_MAX); continue; }
+                if (!ok) { lam = fminf(4.f * lam, IK_LAMBDA_MAX); continue; }
                 // y = A^-1 (e or J^T e): L w = ., L^T y = w
                 for (int i = 0; i < m; ++i) {
                     float s = task ? e[i * T] : y[i * T];
@@ -313,19 +270,19 @@ inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmA
                     } else {
                         s = y[u * T];
                     }
-                    qt[c * T] = clamp_joint_m(qc[c * T] + s, s_lim, n, c, limits);
+                    qt[c * T] = clamp_joint(qc[c * T] + s, s_lim, n, c, limits);
                 }
             }
             bool within;
             const float Et = evaluate_multi<POSE>(P, s_tab, q_rows + dst * nT, j_rows + dst * JT, e_rows + dst * M * T, jscr, st,
                                                   tgt, T, args.pos_tol, args.rot_tol, within);
             if (it < 0 || Et < E) {
-                if (it >= 0) lam = fmaxf(0.5f * lam, IKM_LAMBDA_MIN);
+                if (it >= 0) lam = fmaxf(0.5f * lam, IK_LAMBDA_MIN);
                 cur = dst;
                 E = Et;
                 done = within;
             } else {
-                lam = fminf(4.f * lam, IKM_LAMBDA_MAX);
+                lam = fminf(4.f * lam, IK_LAMBDA_MAX);
             }
             if (it < 0) it = 0;
         }
@@ -351,47 +308,29 @@ inverse_kinematics_multi_kernel(const __grid_constant__ IkmProgram P, const IkmA
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <bool POSE>
-static int launch_ikm(const IkmProgram& P, const IkmArgs& args, cudaStream_t stream) {
-    auto kern = inverse_kinematics_multi_kernel<POSE>;
-    static cudaFuncAttributes attr_by_dev[64];
-    static size_t configured_by_dev[64] = {0};
-    static bool queried_by_dev[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!queried_by_dev[dev & 63]) {
-        cudaError_t e = cudaFuncGetAttributes(&attr_by_dev[dev & 63], kern);
-        if (e != cudaSuccess) { set_error("cudaFuncGetAttributes: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        queried_by_dev[dev & 63] = true;
-    }
-    const size_t static_bytes = attr_by_dev[dev & 63].sharedSizeBytes;
+// the largest power-of-two tile <= 64 rows while two CTAs still fit an SM, else down to one row per CTA
+static TileChoice ikm_tile(const UnionProgram& P, bool pose, size_t static_bytes) {
     const MultiProgram& W = P.walk;
-    auto bytes_of = [&](int T) {
-        return (size_t)IkmSmemLayout(T, W.n_dofs, P.n_u, W.n_ee, POSE, W.n_steps, W.n_jslots, W.n_state_slots).total_floats *
+    return tile_ladder([&](int T) {
+        return (size_t)IkmSmemLayout(T, W.n_dofs, P.n_u, W.n_ee, pose, W.n_steps, W.n_jslots, W.n_state_slots).total_floats *
                sizeof(float);
-    };
-    // the largest power-of-two tile <= 64 rows while two CTAs still fit an SM, else down to one row per CTA
-    int T = 64;
-    while (T > 1 && bytes_of(T) + static_bytes > 113 * 1024) T >>= 1;
-    const size_t smem_bytes = bytes_of(T);
-    if (smem_bytes + static_bytes > 227 * 1024) {
+    }, static_bytes);
+}
+
+template <bool POSE>
+static int launch_ikm(const UnionProgram& P, const IkmArgs& args, cudaStream_t stream) {
+    constexpr auto kern = inverse_kinematics_multi_kernel<POSE>;
+    size_t static_bytes;
+    const int rc = static_smem_bytes<kern>(&static_bytes);
+    if (rc != DRMB200_OK) return rc;
+    const TileChoice c = ikm_tile(P, POSE, static_bytes);
+    if (c.bytes + static_bytes > SMEM_CTA_MAX) {
         set_error("multi-link inverse kinematics needs %zu B of shared memory per CTA (> 227 KB) for one row (%d joints, %d links)",
-                  smem_bytes + static_bytes, W.n_dofs, W.n_ee);
+                  c.bytes + static_bytes, P.walk.n_dofs, P.walk.n_ee);
         return DRMB200_ELIMIT;
     }
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    kern<<<(unsigned)tiles, T, smem_bytes, stream>>>(P, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("multi-link inverse kinematics launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return launch_kernel<kern>((args.batch + c.tile - 1) / c.tile, c.tile, c.bytes, stream, false, "multi-link inverse kinematics", P,
+                               args);
 }
 
 int inverse_kinematics_multi_device(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
@@ -399,8 +338,8 @@ int inverse_kinematics_multi_device(const drmb200_topology_t* topo, int32_t n_ee
                                     const float* upper, const float* damping_in, int64_t batch, int32_t max_iters,
                                     float damping_init, float pos_tol, float rot_tol, float* q, float* pos_err, float* rot_err,
                                     uint8_t* converged, float* damping_out, cudaStream_t stream) {
-    IkmProgram P;
-    const int rc = build_multi_program(topo, n_ee, ee_links, &P.walk);
+    UnionProgram P;
+    const int rc = build_union_program(topo, n_ee, ee_links, &P);
     if (rc != DRMB200_OK) return rc;
     const MultiProgram& W = P.walk;
     if (W.n_dofs == 0) { set_error("inverse kinematics of a model without movable joints"); return DRMB200_EINVAL; }
@@ -412,20 +351,9 @@ int inverse_kinematics_multi_device(const drmb200_topology_t* topo, int32_t n_ee
             return DRMB200_EINVAL;
         }
     }
-    P.n_u = 0;
-    for (int k = 0; k < W.n_steps; ++k)
-        if (W.dof[k] >= 0) P.u_dof[P.n_u++] = W.dof[k];
-    if (max_iters < 0) { set_error("max_iters=%d < 0", max_iters); return DRMB200_EINVAL; }
-    if (!(pos_tol >= 0.f) || !(rot_tol >= 0.f)) { set_error("tolerances must be >= 0 (pos_tol=%g, rot_tol=%g)", pos_tol, rot_tol); return DRMB200_EINVAL; }
-    if ((lower == nullptr) != (upper == nullptr)) { set_error("lower and upper must both be given or both be null"); return DRMB200_EINVAL; }
-    if (!(damping_init > 0.f)) { set_error("damping_init=%g must be > 0", damping_init); return DRMB200_EINVAL; }
-    if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
-    if (batch == 0) return DRMB200_OK;
-    if (table == nullptr || q0 == nullptr || target_pos == nullptr || q == nullptr || pos_err == nullptr || rot_err == nullptr ||
-        converged == nullptr || damping_out == nullptr) {
-        set_error("null pointer argument");
-        return DRMB200_EINVAL;
-    }
+    const int arg_rc = check_ik_arguments(table, q0, target_pos, lower, upper, batch, max_iters, damping_init, pos_tol, rot_tol, q,
+                                          pos_err, rot_err, converged, damping_out);
+    if (arg_rc != DRMB200_OK || batch == 0) return arg_rc;
     IkmArgs args;
     args.table = table; args.q0 = q0; args.tpos = target_pos; args.tquat = target_quat;
     args.lower = lower; args.upper = upper; args.damping_in = damping_in;

@@ -14,7 +14,7 @@
 // so that every store of a warp is one contiguous 128-byte line (threads = consecutive configurations): no staging
 // needed for the outputs.  q / qd tiles are staged through shared memory like everywhere else.
 // Algorithmic bytes per configuration: 4n (+4n) in, n_links * (48 [+16] [+24]) out.
-#include "drm_common.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -157,25 +157,13 @@ int kinematic_state_device(const drmb200_topology_t* topo, const float* table, c
     const bool with_vel = vels != nullptr;
     KsArgs args;
     args.table = table; args.q = q; args.qd = qd; args.poses = poses; args.quats = quats; args.vels = vels; args.batch = batch;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd)) ? 1 : 0;
+    args.aligned = aligned16(q, qd);
     const KsSmem L(prog.n_dofs, prog.n_links, prog.n_slots, with_vel);
     const size_t smem_bytes = (size_t)L.total_floats * sizeof(float);
-    if (smem_bytes > 227 * 1024) { set_error("kinematic state kernel needs %zu B of shared memory (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
+    if (smem_bytes > SMEM_CTA_MAX) { set_error("kinematic state kernel needs %zu B of shared memory (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (batch + KS_TILE - 1) / KS_TILE;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    cudaError_t e;
-    if (with_vel) {
-        e = cudaFuncSetAttribute(kinematic_state_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e == cudaSuccess) kinematic_state_kernel<true><<<(unsigned)tiles, KS_TILE, smem_bytes, stream>>>(prog, args);
-    } else {
-        e = cudaFuncSetAttribute(kinematic_state_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e == cudaSuccess) kinematic_state_kernel<false><<<(unsigned)tiles, KS_TILE, smem_bytes, stream>>>(prog, args);
-    }
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("kinematic_state launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return with_vel ? launch_kernel<kinematic_state_kernel<true>>(tiles, KS_TILE, smem_bytes, stream, false, "kinematic_state", prog, args)
+                    : launch_kernel<kinematic_state_kernel<false>>(tiles, KS_TILE, smem_bytes, stream, false, "kinematic_state", prog, args);
 }
 
 }  // namespace drm

@@ -14,7 +14,7 @@
 //
 // Algorithmic HBM bytes per configuration: 4n in + 4n^2 out (224 B at n = 7); about 1 k instructions per column and
 // 7-DoF configuration, FP32-issue-bound like RNEA.
-#include "drm_common.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -163,51 +163,26 @@ mass_matrix_kernel(const __grid_constant__ TreeProgram prog, const __grid_consta
     }
 }
 
-template <int T>
-static int launch_mm(const TreeProgram& prog, const FoldProgram& fold, const MmArgs& args, size_t smem_bytes, cudaStream_t stream) {
-    static size_t configured_by_dev[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(mass_matrix_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    mass_matrix_kernel<T><<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, fold, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("mass matrix launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
-}
-
 // prefolded: `table` holds the rows of drmb200_fold_link_table (constant models fold once instead of once per CTA)
 int mass_matrix_device_impl(const drmb200_topology_t* topo, const float* table, const float* q, int64_t batch, float* H,
                             cudaStream_t stream, bool prefolded) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    if (prefolded && !cp->foldable) { set_error("this topology has no link behind a fixed joint to fold"); return DRMB200_EINVAL; }
-    // "rnea_fold": walk only the movable links (fixed links folded into their movable ancestors while the table is staged)
-    const bool folded = prefolded || (cp->foldable && get_option(11) != 0);
-    const TreeProgram& prog = folded ? cp->red : cp->full;
-    FoldProgram fold = cp->fold;
-    if (!folded) fold.n_red = 0;                        // the kernel's "no folding" flag
-    if (prefolded) fold.n_full = 0;                     // ... and its "rows are folded already" flag
+    FoldChoice fc;
+    const int rc = select_fold(topo, prefolded, &fc);
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
     if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
     if (batch == 0 || prog.n_dofs == 0) return DRMB200_OK;
     if (table == nullptr || q == nullptr || H == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
     MmArgs args;
     args.table = table; args.q = q; args.H = H; args.batch = batch;
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(H)) ? 1 : 0;
-    auto bytes_of = [&](int T) { return (size_t)MmSmemLayout(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float); };
-    const int tile = bytes_of(64) <= 113 * 1024 ? 64 : 32;
-    const size_t smem_bytes = bytes_of(tile);
-    if (smem_bytes > 227 * 1024) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
-    return tile == 64 ? launch_mm<64>(prog, fold, args, smem_bytes, stream) : launch_mm<32>(prog, fold, args, smem_bytes, stream);
+    args.aligned = aligned16(q, H);
+    const TileChoice c = tile_64_or_32([&](int T) {
+        return (size_t)MmSmemLayout(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float);
+    });
+    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
+    const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    return c.tile == 64 ? launch_kernel<mass_matrix_kernel<64>>(tiles, 64, c.bytes, stream, false, "mass matrix", prog, fc.fold, args)
+                        : launch_kernel<mass_matrix_kernel<32>>(tiles, 32, c.bytes, stream, false, "mass matrix", prog, fc.fold, args);
 }
 
 int mass_matrix_device(const drmb200_topology_t* topo, const float* table, const float* q, int64_t batch, float* H, cudaStream_t stream) {

@@ -31,4 +31,34 @@ struct MultiProgram {
 // index out of range or a link requested twice.
 int build_multi_program(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, MultiProgram* prog);
 
+// The walk as the solver kernels (multi-link inverse kinematics, operational-space dynamics) use it, with U: the movable
+// joints on the union of the paths, which span the columns of their stacked Jacobian.
+struct UnionProgram {
+    MultiProgram walk;
+    int32_t n_u;                           // movable joints on the union of the paths
+    int8_t u_dof[DRMB200_MAX_LINKS];       // U column -> q / dof column, in walk order
+};
+
+// build_multi_program, then U (fk_tree.cu)
+int build_union_program(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, UnionProgram* prog);
+
+// Link l's rows of a stacked Jacobian J [MR n_ee][n_u] (one row's slot-major slots, rows n_u T apart): J_lin = z x p_e -
+// z x p_j over J_ang = z (MR = 6 only), from the walk's joint scratch jscr (z, z x p_j per path depth) and the link's
+// position p_e.  Columns of joints off the link's path are left as they are (zero).
+__device__ __forceinline__ void link_jacobian(const UnionProgram& P, int l, int MR, V3 p, const float* jscr, float* J, int T) {
+    const int n_u = P.n_u;
+    const int rs = n_u * T;
+    float* Jl = J + MR * l * rs;
+    for (int u = 0; u < n_u; ++u) {
+        const int s = P.walk.cslot[l][P.u_dof[u]];
+        if (s < 0) continue;
+        const float* js = jscr + s * 6 * T;
+        const V3 z = ldv(js, T), m = ldv(js + 3 * T, T);
+        const V3 j = cross_add(z, p, v3(-m.x, -m.y, -m.z));
+        float* col = Jl + u * T;
+        col[0] = j.x; col[rs] = j.y; col[2 * rs] = j.z;
+        if (MR == 6) { col[3 * rs] = z.x; col[4 * rs] = z.y; col[5 * rs] = z.z; }
+    }
+}
+
 }  // namespace drm

@@ -32,17 +32,12 @@
 // [M].  The output tiles are written back with a cooperative transposing copy: consecutive threads store consecutive floats
 // of the contiguous [T, M, M] block, so the stores coalesce without a second row-major copy of the tile in shared memory.
 #include "aba_body.cuh"
+#include "launch.cuh"
 #include "multi_program.cuh"
 
 namespace drm {
 
 constexpr int OSD_STATE = 24;          // floats of a spilled branch state: R (9), p, omega, v, alpha, a
-
-struct OsdProgram {
-    MultiProgram walk;
-    int32_t n_u;                       // movable joints on the union of the paths
-    int8_t u_dof[DRMB200_MAX_LINKS];   // U column -> q / dof column, in walk order
-};
 
 struct OsdArgs {
     const float* __restrict__ table;
@@ -62,7 +57,7 @@ struct OsdArgs {
 struct OsdSmemLayout {
     AbaSmemLayout aba;
     int jac, jscr, state, vel, bias, acc, inv, total_floats;
-    __host__ __device__ OsdSmemLayout(int T, const TreeProgram& tp, const OsdProgram& P, int M)
+    __host__ __device__ OsdSmemLayout(int T, const TreeProgram& tp, const UnionProgram& P, int M)
         : aba(T, tp.n_dofs, tp.n_links, tp.n_slots) {
         int o = aba.total_floats;
         jac = o;   o += M * P.n_u * T;
@@ -79,11 +74,9 @@ struct OsdSmemLayout {
 // The kinematic walk of one row: J [M][n_u], velocity and bias [M] (this row's slot-major slots; entries of links that are
 // not walked -- the root -- and of joints off a link's path are left as staged: zero).  qrow / qdrow: the row's q, qd.
 template <int T>
-__device__ __forceinline__ void osd_walk(const OsdProgram& P, const float* s_tab, const float* qrow, const float* qdrow, int MR,
+__device__ __forceinline__ void osd_walk(const UnionProgram& P, const float* s_tab, const float* qrow, const float* qdrow, int MR,
                                          float* J, float* vel, float* bias, float* jscr, float* st) {
     const MultiProgram& W = P.walk;
-    const int n_u = P.n_u;
-    const int rs = n_u * T;                  // stride between rows of J
     const V3 zero = v3(0.f, 0.f, 0.f);
     M3 R = identity3();
     V3 p = zero, w = zero, v = zero, A = zero, a = zero;
@@ -124,18 +117,8 @@ __device__ __forceinline__ void osd_walk(const OsdProgram& P, const float* s_tab
         }
         const int l = W.ee[k];
         if (l < 0) continue;
-        // link l: its rows of J (J_lin = z x p_e - z x p_j over J_ang = z), of J qd and of Jdot qd
-        float* Jl = J + MR * l * rs;
-        for (int u = 0; u < n_u; ++u) {
-            const int s = W.cslot[l][P.u_dof[u]];
-            if (s < 0) continue;             // off this link's path: stays zero
-            const float* js = jscr + s * 6 * T;
-            const V3 z = ldv(js, T), m = ldv(js + 3 * T, T);
-            const V3 j = cross_add(z, p, v3(-m.x, -m.y, -m.z));
-            float* col = Jl + u * T;
-            col[0] = j.x; col[rs] = j.y; col[2 * rs] = j.z;
-            if (MR == 6) { col[3 * rs] = z.x; col[4 * rs] = z.y; col[5 * rs] = z.z; }
-        }
+        // link l: its rows of J, of J qd and of Jdot qd
+        link_jacobian(P, l, MR, p, jscr, J, T);
         stv(vel + MR * l * T, T, v);
         stv(bias + MR * l * T, T, a);
         if (MR == 6) { stv(vel + (MR * l + 3) * T, T, w); stv(bias + (MR * l + 3) * T, T, A); }
@@ -229,7 +212,7 @@ __device__ __forceinline__ void store_transposed(float* dst, const float* src, i
 
 template <int T>
 __global__ void __launch_bounds__(T)
-operational_space_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ OsdProgram P, const OsdArgs args) {
+operational_space_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ UnionProgram P, const OsdArgs args) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar;
 
@@ -331,26 +314,9 @@ operational_space_kernel(const __grid_constant__ TreeProgram prog, const __grid_
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <int T>
-static int launch_osd_tile(const TreeProgram& prog, const OsdProgram& P, const OsdArgs& args, size_t smem_bytes,
-                           cudaStream_t stream) {
-    auto kern = operational_space_kernel<T>;
-    static size_t configured_by_dev[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    kern<<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, P, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("operational-space dynamics launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+// the largest power-of-two tile <= 64 rows while two CTAs still fit an SM, else down to one row per CTA
+static TileChoice osd_tile(const TreeProgram& prog, const UnionProgram& P, int M, size_t static_bytes) {
+    return tile_ladder([&](int T) { return (size_t)OsdSmemLayout(T, prog, P, M).total_floats * sizeof(float); }, static_bytes);
 }
 
 int operational_space_dynamics_device(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
@@ -359,8 +325,8 @@ int operational_space_dynamics_device(const drmb200_topology_t* topo, int32_t n_
                                       float* bias_acceleration, cudaStream_t stream) {
     if (n_ee < 1 || n_ee > MT_MAX_EE) { set_error("n_ee=%d outside [1, %d]", n_ee, MT_MAX_EE); return DRMB200_EINVAL; }
     if (ee_links == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
-    OsdProgram P;
-    int rc = build_multi_program(topo, n_ee, ee_links, &P.walk);
+    UnionProgram P;
+    int rc = build_union_program(topo, n_ee, ee_links, &P);
     if (rc != DRMB200_OK) return rc;
     const CachedPrograms* cp = cached_programs(topo, &rc);
     if (cp == nullptr) return rc;
@@ -373,39 +339,37 @@ int operational_space_dynamics_device(const drmb200_topology_t* topo, int32_t n_
         set_error("null pointer argument");
         return DRMB200_EINVAL;
     }
-    const MultiProgram& W = P.walk;
-    P.n_u = 0;
-    for (int k = 0; k < W.n_steps; ++k)
-        if (W.dof[k] >= 0) P.u_dof[P.n_u++] = W.dof[k];
 
     OsdArgs args;
     args.table = table; args.q = q; args.qd = qd; args.f = f;
     args.inv_inertia = inv_inertia; args.acceleration = acceleration; args.velocity = velocity; args.bias = bias_acceleration;
     args.batch = batch; args.flags = flags & (DRMB200_GRAVITY | DRMB200_DAMPING);
     args.M = (position_only ? 3 : 6) * n_ee;
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd) && al16(f)) ? 1 : 0;
+    args.aligned = aligned16(q, qd, f);
 
-    // the largest power-of-two tile <= 64 rows while two CTAs still fit an SM, else down to one row per CTA
-    auto bytes_of = [&](int T) { return (size_t)OsdSmemLayout(T, prog, P, args.M).total_floats * sizeof(float); };
-    constexpr size_t STATIC_BYTES = 128;        // static shared memory of every instantiation (-Xptxas -v)
-    int T = 64;
-    while (T > 1 && bytes_of(T) + STATIC_BYTES > 113 * 1024) T >>= 1;
-    const size_t smem_bytes = bytes_of(T);
-    if (smem_bytes + STATIC_BYTES > 227 * 1024) {
+    // every instantiation declares the same static shared memory (the mbarrier)
+    size_t static_bytes;
+    rc = static_smem_bytes<operational_space_kernel<64>>(&static_bytes);
+    if (rc != DRMB200_OK) return rc;
+    const TileChoice c = osd_tile(prog, P, args.M, static_bytes);
+    if (c.bytes + static_bytes > SMEM_CTA_MAX) {
         set_error("operational-space dynamics needs %zu B of shared memory per CTA (> 227 KB) for one row (%d joints, %d links, M = %d)",
-                  smem_bytes + STATIC_BYTES, prog.n_dofs, prog.n_links, args.M);
+                  c.bytes + static_bytes, prog.n_dofs, prog.n_links, args.M);
         return DRMB200_ELIMIT;
     }
-    switch (T) {
-        case 64: return launch_osd_tile<64>(prog, P, args, smem_bytes, stream);
-        case 32: return launch_osd_tile<32>(prog, P, args, smem_bytes, stream);
-        case 16: return launch_osd_tile<16>(prog, P, args, smem_bytes, stream);
-        case 8: return launch_osd_tile<8>(prog, P, args, smem_bytes, stream);
-        case 4: return launch_osd_tile<4>(prog, P, args, smem_bytes, stream);
-        case 2: return launch_osd_tile<2>(prog, P, args, smem_bytes, stream);
-        default: return launch_osd_tile<1>(prog, P, args, smem_bytes, stream);
+    const int64_t tiles = (batch + c.tile - 1) / c.tile;
+#define DRM_LAUNCH_OSD(TT) \
+    launch_kernel<operational_space_kernel<TT>>(tiles, TT, c.bytes, stream, false, "operational-space dynamics", prog, P, args)
+    switch (c.tile) {
+        case 64: return DRM_LAUNCH_OSD(64);
+        case 32: return DRM_LAUNCH_OSD(32);
+        case 16: return DRM_LAUNCH_OSD(16);
+        case 8: return DRM_LAUNCH_OSD(8);
+        case 4: return DRM_LAUNCH_OSD(4);
+        case 2: return DRM_LAUNCH_OSD(2);
+        default: return DRM_LAUNCH_OSD(1);
     }
+#undef DRM_LAUNCH_OSD
 }
 
 }  // namespace drm

@@ -29,11 +29,11 @@
 // 2 kflop per 7-DoF configuration the kernel is FP32-issue-bound, not HBM-bound (SURVEY.md 8d).
 #include <cstdlib>
 #include <cstring>
-#include "drm_common.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
-// configurations per CTA: template parameter T of the kernel, 64 or 128 (see inverse_dynamics_device)
+// configurations per CTA: template parameter T of the kernel, 64 or 128 (see rnea_tile)
 constexpr float GRAVITY = 9.81f;     // robot_model.py:347
 
 struct RneaArgs {
@@ -381,26 +381,10 @@ int build_tree_program(const drmb200_topology_t* topo, TreeProgram* prog) {
 
 template <int T, bool PACKED, bool DUMP, bool FOLD>
 static int launch_rnea(const TreeProgram& prog, const FoldProgram& fold, const RneaArgs& args, cudaStream_t stream) {
-    const RneaSmemLayout L(T, prog.n_dofs, prog.n_links, prog.n_slots);
-    const size_t smem_bytes = (size_t)L.total_floats * sizeof(float);
-    if (smem_bytes > 227 * 1024) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    auto kern = rnea_kernel<T, PACKED, DUMP, FOLD>;
-    static size_t configured_by_dev[64] = {0};     // per instantiation, per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    kern<<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, fold, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("rnea launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    const size_t smem_bytes = (size_t)RneaSmemLayout(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float);
+    if (smem_bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
+    return launch_kernel<rnea_kernel<T, PACKED, DUMP, FOLD>>((args.batch + T - 1) / T, T, smem_bytes, stream, false, "rnea", prog,
+                                                             fold, args);
 }
 
 // the tree program (and the folded one) depend only on the topology: keep the last two per thread
@@ -463,6 +447,19 @@ const CachedPrograms* cached_programs(const drmb200_topology_t* topo, int* rc_ou
     return &c;
 }
 
+int select_fold(const drmb200_topology_t* topo, bool prefolded, FoldChoice* out) {
+    int rc;
+    const CachedPrograms* cp = cached_programs(topo, &rc);
+    if (cp == nullptr) return rc;
+    if (prefolded && !cp->foldable) { set_error("this topology has no link behind a fixed joint to fold"); return DRMB200_EINVAL; }
+    out->folded = prefolded || (cp->foldable && get_option(11) != 0);      // "rnea_fold"
+    out->prog = out->folded ? &cp->red : &cp->full;
+    out->fold = cp->fold;
+    if (!out->folded) out->fold.n_red = 0;
+    if (prefolded) out->fold.n_full = 0;
+    return DRMB200_OK;
+}
+
 // The folded canonical table of a link table, once, for callers whose table does not change between launches (constant
 // models): folding it while staging costs every CTA a noticeable share of the inverse-dynamics kernel, a plain copy of
 // n_red x 28 floats costs nothing.  Output: [n_red, 28] canonical rows (row 0 unused).
@@ -478,10 +475,10 @@ fold_table_kernel(const __grid_constant__ TreeProgram prog, const __grid_constan
 }
 
 int64_t folded_table_rows(const drmb200_topology_t* topo) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    return (cp->foldable && get_option(11) != 0) ? cp->fold.n_red : 0;
+    FoldChoice fc;
+    const int rc = select_fold(topo, false, &fc);
+    if (rc != DRMB200_OK) return rc;
+    return fc.folded ? fc.fold.n_red : 0;
 }
 
 int fold_table_device(const drmb200_topology_t* topo, const float* table, float* folded, cudaStream_t stream) {
@@ -491,68 +488,54 @@ int fold_table_device(const drmb200_topology_t* topo, const float* table, float*
     if (!cp->foldable) { set_error("this topology has no link behind a fixed joint to fold (drmb200_folded_table_rows() == 0)"); return DRMB200_EINVAL; }
     if (table == nullptr || folded == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
     const size_t smem = (size_t)(cp->fold.n_red * DRMB200_TABLE_STRIDE + cp->fold.n_full * 40) * sizeof(float);
-    fold_table_kernel<<<1, 64, smem, stream>>>(cp->red, cp->fold, table, folded);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("fold_table launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
+    return launch_kernel<fold_table_kernel>(1, 64, smem, stream, false, "fold_table", cp->red, cp->fold, table, folded);
 }
 
-// inverse dynamics from a table folded beforehand (drmb200_fold_link_table)
-int inverse_dynamics_prefolded_device(const drmb200_topology_t* topo, const float* folded, const float* q, const float* qd,
-                                      const float* qdd, int64_t batch, uint32_t flags, float* tau, cudaStream_t stream) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    if (!cp->foldable) { set_error("this topology has no link behind a fixed joint to fold"); return DRMB200_EINVAL; }
-    if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
-    if (batch == 0 || cp->red.n_dofs == 0) return DRMB200_OK;
-    if (folded == nullptr || q == nullptr || qd == nullptr || qdd == nullptr || tau == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
-    const TreeProgram* prog = &cp->red;
+// Tile: 128 amortises the table staging (heavier since it folds the fixed links) over twice the configurations (chosen by a
+// Panda sweep before the H100 port; not re-measured on the H100); 64 only for batches that would leave SMs without a CTA,
+// and for models whose 128-row footprint is larger than RNEA_128_MAX_BYTES.  "rnea_tile" 64 / 128 forces one (256 lost that
+// sweep too).
+constexpr size_t RNEA_128_MAX_BYTES = 110 * 1024;
+
+static int rnea_tile(const TreeProgram& prog, int64_t batch) {
     int tile = (batch < 32768) ? 64 : 128;
     if (get_option(12) == 64 || get_option(12) == 128) tile = get_option(12);
-    if ((size_t)RneaSmemLayout(128, prog->n_dofs, prog->n_links, prog->n_slots).total_floats * sizeof(float) > 110 * 1024) tile = 64;
+    if ((size_t)RneaSmemLayout(128, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float) > RNEA_128_MAX_BYTES) tile = 64;
+    return tile;
+}
+
+template <bool FOLD>
+static int launch_rnea_tile(int tile, const TreeProgram& prog, const FoldProgram& fold, const RneaArgs& args, cudaStream_t stream) {
+    const bool packed = get_option(4) != 0;             // "rnea_packed": f32x2 pair arithmetic (default) vs scalar, for A/B runs
+    if (tile == 64) return packed ? launch_rnea<64, true, false, FOLD>(prog, fold, args, stream) : launch_rnea<64, false, false, FOLD>(prog, fold, args, stream);
+    return packed ? launch_rnea<128, true, false, FOLD>(prog, fold, args, stream) : launch_rnea<128, false, false, FOLD>(prog, fold, args, stream);
+}
+
+// prefolded: `table` holds the rows of drmb200_fold_link_table
+static int inverse_dynamics_impl(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
+                                 const float* qdd, int64_t batch, uint32_t flags, float* tau, cudaStream_t stream, bool prefolded) {
+    FoldChoice fc;
+    const int rc = select_fold(topo, prefolded, &fc);
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
+    if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
+    if (batch == 0 || prog.n_dofs == 0) return DRMB200_OK;
+    if (table == nullptr || q == nullptr || qd == nullptr || qdd == nullptr || tau == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
     RneaArgs args;
-    args.table = folded; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau; args.batch = batch; args.flags = flags;
+    args.table = table; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau; args.batch = batch; args.flags = flags;
     args.vels = args.accs = args.forces = nullptr;
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd) && al16(qdd) && al16(tau)) ? 1 : 0;
-    FoldProgram pre = cp->fold;
-    pre.n_full = 0;                                       // the kernel's "rows are folded already" flag
-    const bool packed = get_option(4) != 0;
-    if (tile == 64) return packed ? launch_rnea<64, true, false, true>(*prog, pre, args, stream) : launch_rnea<64, false, false, true>(*prog, pre, args, stream);
-    return packed ? launch_rnea<128, true, false, true>(*prog, pre, args, stream) : launch_rnea<128, false, false, true>(*prog, pre, args, stream);
+    args.aligned = aligned16(q, qd, qdd, tau);
+    const int tile = rnea_tile(prog, batch);
+    return fc.folded ? launch_rnea_tile<true>(tile, prog, fc.fold, args, stream) : launch_rnea_tile<false>(tile, prog, fc.fold, args, stream);
 }
 
 int inverse_dynamics_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                             const float* qdd, int64_t batch, uint32_t flags, float* tau, cudaStream_t stream) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
-    if (batch == 0 || cp->full.n_dofs == 0) return DRMB200_OK;
-    if (table == nullptr || q == nullptr || qd == nullptr || qdd == nullptr || tau == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
-    // "rnea_fold" (default on): walk only the movable links, fixed links folded into their movable ancestors at staging time
-    const bool fold = cp->foldable && get_option(11) != 0;
-    const TreeProgram* prog = fold ? &cp->red : &cp->full;
-    // tile: 128 amortises the table staging (heavier since it folds the fixed links) over twice the configurations
-    // (chosen by a Panda sweep before the H100 port; not re-measured on the H100); 64 only for batches that would leave
-    // SMs without a CTA, and for models whose 128-row footprint is too big
-    int tile = (batch < 32768) ? 64 : 128;
-    if (get_option(12) == 64 || get_option(12) == 128) tile = get_option(12);      // 256 lost that sweep too
-    if ((size_t)RneaSmemLayout(128, prog->n_dofs, prog->n_links, prog->n_slots).total_floats * sizeof(float) > 110 * 1024) tile = 64;
-    RneaArgs args;
-    args.table = table; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau; args.batch = batch; args.flags = flags;
-    args.vels = args.accs = args.forces = nullptr;
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd) && al16(qdd) && al16(tau)) ? 1 : 0;
-    const bool packed = get_option(4) != 0;             // "rnea_packed": f32x2 pair arithmetic (default) vs scalar, for A/B runs
-    if (fold) {
-        if (tile == 64) return packed ? launch_rnea<64, true, false, true>(*prog, cp->fold, args, stream) : launch_rnea<64, false, false, true>(*prog, cp->fold, args, stream);
-        return packed ? launch_rnea<128, true, false, true>(*prog, cp->fold, args, stream) : launch_rnea<128, false, false, true>(*prog, cp->fold, args, stream);
-    }
-    if (tile == 64) return packed ? launch_rnea<64, true, false, false>(*prog, cp->fold, args, stream) : launch_rnea<64, false, false, false>(*prog, cp->fold, args, stream);
-    return packed ? launch_rnea<128, true, false, false>(*prog, cp->fold, args, stream) : launch_rnea<128, false, false, false>(*prog, cp->fold, args, stream);
+    return inverse_dynamics_impl(topo, table, q, qd, qdd, batch, flags, tau, stream, false);
+}
+int inverse_dynamics_prefolded_device(const drmb200_topology_t* topo, const float* folded, const float* q, const float* qd,
+                                      const float* qdd, int64_t batch, uint32_t flags, float* tau, cudaStream_t stream) {
+    return inverse_dynamics_impl(topo, folded, q, qd, qdd, batch, flags, tau, stream, true);
 }
 
 // inverse dynamics + the per-link state of the reference's bodies (vel, acc, force), see rnea_kernel<.., DUMP>
@@ -569,8 +552,7 @@ int dynamic_state_device(const drmb200_topology_t* topo, const float* table, con
     RneaArgs args;
     args.table = table; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau; args.batch = batch; args.flags = flags;
     args.vels = vels; args.accs = accs; args.forces = forces;
-    auto al16 = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    args.aligned = (al16(q) && al16(qd) && al16(qdd) && al16(tau)) ? 1 : 0;
+    args.aligned = aligned16(q, qd, qdd, tau);
     return launch_rnea<64, true, true, false>(*prog, cp->fold, args, stream);
 }
 

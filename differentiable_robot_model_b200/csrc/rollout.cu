@@ -24,6 +24,7 @@
 // the pre-update of step t; the table gradient of all steps is summed in the adjoint's per-CTA partial tables and reduced
 // once, so a backward is 2T + 2 launches.
 #include "aba_body.cuh"
+#include "launch.cuh"
 
 namespace drm {
 
@@ -207,39 +208,13 @@ __global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStep
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <int T>
-static int launch_rollout(const TreeProgram& prog, const FoldProgram& fold, const RolloutArgs& args, size_t smem_bytes,
-                          cudaStream_t stream) {
-    static size_t configured_by_dev[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    size_t& configured = configured_by_dev[dev & 63];
-    if (smem_bytes > configured) {
-        cudaError_t e = cudaFuncSetAttribute(rollout_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu B smem): %s", smem_bytes, cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        configured = smem_bytes;
-    }
-    const int64_t tiles = (args.batch + T - 1) / T;
-    if (tiles > 0x7fffffffLL) { set_error("batch too large for one launch"); return DRMB200_EINVAL; }
-    rollout_kernel<T><<<(unsigned)tiles, T, smem_bytes, stream>>>(prog, fold, args);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("rollout launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-    count_launch();
-    return DRMB200_OK;
-}
-
-static bool al16(const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
                                     const float* f, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q,
                                     float* qd, float* qdd, cudaStream_t stream) {
-    int rc;
-    const CachedPrograms* cp = cached_programs(topo, &rc);
-    if (cp == nullptr) return rc;
-    const bool folded = cp->foldable && get_option(11) != 0;          // "rnea_fold", as drmb200_forward_dynamics
-    const TreeProgram& prog = folded ? cp->red : cp->full;
-    FoldProgram fold = cp->fold;
-    if (!folded) fold.n_red = 0;
+    FoldChoice fc;
+    const int rc = select_fold(topo, false, &fc);                   // "rnea_fold", as drmb200_forward_dynamics
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
     if (batch == 0 || n_steps == 0 || prog.n_dofs == 0) return DRMB200_OK;
     if (table == nullptr || q0 == nullptr || qd0 == nullptr || f == nullptr || q == nullptr || qd == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
@@ -247,15 +222,17 @@ int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float*
     RolloutArgs args;
     args.table = table; args.q0 = q0; args.qd0 = qd0; args.f = f; args.q = q; args.qd = qd; args.qdd = qdd;
     args.batch = batch; args.n_steps = n_steps; args.dt = dt; args.flags = flags;
-    args.aligned = (al16(q0) && al16(qd0) && al16(f) && al16(q) && al16(qd) && al16(qdd) && ((batch * prog.n_dofs) & 3) == 0) ? 1 : 0;
+    args.aligned = aligned16(q0, qd0, f, q, qd, qdd) && ((batch * prog.n_dofs) & 3) == 0;
 
     // 64 configurations per CTA when that still gives every SM a CTA and the per-link state leaves room for two CTAs per
     // SM; 32 otherwise -- rollout batches are often below one wave of 64-thread CTAs, and a CTA stays resident for all steps
-    auto bytes_of = [&](int T) { return (size_t)RolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float); };
-    const int tile = (bytes_of(64) <= 113 * 1024 && (batch + 63) / 64 >= device_sm_count()) ? 64 : 32;
-    const size_t smem_bytes = bytes_of(tile);
-    if (smem_bytes > 227 * 1024) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", smem_bytes); return DRMB200_ELIMIT; }
-    return tile == 64 ? launch_rollout<64>(prog, fold, args, smem_bytes, stream) : launch_rollout<32>(prog, fold, args, smem_bytes, stream);
+    const TileChoice c = tile_64_or_32([&](int T) {
+        return (size_t)RolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float);
+    }, 0, (batch + 63) / 64 >= device_sm_count());
+    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
+    const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    return c.tile == 64 ? launch_kernel<rollout_kernel<64>>(tiles, 64, c.bytes, stream, false, "rollout", prog, fc.fold, args)
+                        : launch_kernel<rollout_kernel<32>>(tiles, 32, c.bytes, stream, false, "rollout", prog, fc.fold, args);
 }
 
 static int64_t round256(int64_t bytes) { return (bytes + 255) & ~(int64_t)255; }
@@ -295,11 +272,7 @@ int forward_dynamics_rollout_backward_device(const drmb200_topology_t* topo, con
     int64_t blocks = (count + 255) / 256;
     if (blocks > (int64_t)device_sm_count() * 8) blocks = (int64_t)device_sm_count() * 8;
     auto step_kernel = [&](const AdjStepArgs& a) {
-        rollout_adjoint_step_kernel<<<(unsigned)blocks, 256, 0, stream>>>(a);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { set_error("rollout adjoint step launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
-        count_launch();
-        return DRMB200_OK;
+        return launch_kernel<rollout_adjoint_step_kernel>(blocks, 256, 0, stream, false, "rollout adjoint step", a);
     };
 
     AdjStepArgs a = {};

@@ -1,14 +1,13 @@
-// Host-side check (no GPU needed): the tile each of four kernels picks for a model, from the real program builders and the
-// real __host__ __device__ shared-memory layout structs.
+// Host-side check (no GPU needed): the tile each of four kernels picks for a model, from the real program builders, the real
+// fold selection and the real tile choosers of the kernels' host code:
 //
-//   dynamics_derivatives.cu     cached_programs -> tree / fold program -> DerivSmemLayout, TC = 128 / n lowered to fit
-//   inverse_kinematics.cu       build_path_program -> IkSmemLayout, T = 64 or 32
-//   inverse_kinematics_multi.cu build_multi_program -> IkmSmemLayout, T = 64, 32, ..., 1
-//   operational_space.cu        build_multi_program + cached_programs (full tree) -> OsdSmemLayout, T = 64, 32, ..., 1
+//   dynamics_derivatives.cu     select_fold -> deriv_tile (DerivSmemLayout, TC = 128 / n lowered to fit)
+//   inverse_kinematics.cu       build_path_program -> ik_tile (IkSmemLayout, T = 64 or 32)
+//   inverse_kinematics_multi.cu build_union_program -> ikm_tile (IkmSmemLayout, T = 64, 32, ..., 1)
+//   operational_space.cu        build_union_program + cached_programs (full tree) -> osd_tile (OsdSmemLayout, T = 64, ..., 1)
 //
-// The choosers live inside the launch functions, next to the launch, so the loops below restate them over the real
-// structs; the static shared bytes the kernels add are the `-Xptxas -v` values (the GPU tests read them back from the
-// device).  tests/test_tile_choice.py compares every line with the Python mirrors of tests/tile_mirrors.py.
+// The static shared bytes the kernels add are the `-Xptxas -v` values (the GPU tests read them back from the device).
+// tests/test_tile_choice.py compares every line with the Python mirrors of tests/tile_mirrors.py.
 //
 // stdin: one case per line: N, N-1 parents, N-1 axis codes (0 = fixed), n_ee, n_ee link indices.
 // stdout: one line per case, eleven "tile bytes" pairs: derivatives ID / FD with folding, ID / FD without folding (the
@@ -26,40 +25,33 @@
 #include "inverse_kinematics_multi.cu"
 #include "operational_space.cu"
 
+static int g_rnea_fold = 0;
+
 namespace drm {
 void set_error(const char*, ...) {}
 void count_launch(int) {}
-int get_option(int) { return 0; }
+int get_option(int which) { return which == 11 ? g_rnea_fold : 0; }       // "rnea_fold"
 }  // namespace drm
 
 using namespace drm;
 
-static constexpr size_t TWO_CTAS = 113 * 1024, CAP = 227 * 1024;
 static constexpr size_t STATIC_DERIV = 128, STATIC_IK = 0, STATIC_IKM = 0, STATIC_OSD = 128;
 
+// a choice as the ELIMIT message states it: dynamic + static bytes, tile 0 when refused
+static void put(TileChoice c, size_t stat) {
+    const size_t b = c.bytes + stat;
+    std::printf(" %d %zu", b > SMEM_CTA_MAX ? 0 : c.tile, b);
+}
 static void put(int tile, size_t bytes) { std::printf(" %d %zu", tile, bytes); }
 
-static void deriv(const CachedPrograms* cp, bool fold, bool prefolded, bool fd) {
-    const bool folded = prefolded || (cp->foldable && fold);
-    if (prefolded && !cp->foldable) { put(DRMB200_EINVAL, 0); return; }
-    const TreeProgram& prog = folded ? cp->red : cp->full;
-    const int fold_full = (folded && !prefolded) ? cp->fold.n_full : 0;
-    const int n = prog.n_dofs;
-    if (n == 0) { put(-1000, 0); return; }          // nothing to launch
-    auto bytes_of = [&](int tc) {
-        return (size_t)DerivSmemLayout(tc, n, prog.n_links, prog.n_slots, fold_full, fd).total_floats * 4 + STATIC_DERIV;
-    };
-    int tc = n >= 128 ? 1 : 128 / n;
-    while (tc > 1 && bytes_of(tc) > TWO_CTAS) --tc;
-    put(bytes_of(tc) > CAP ? 0 : tc, bytes_of(tc));
-}
-
-template <typename F>
-static void ladder(F floats_of, size_t stat) {
-    int T = 64;
-    while (T > 1 && (size_t)floats_of(T) * 4 + stat > TWO_CTAS) T >>= 1;
-    const size_t b = (size_t)floats_of(T) * 4 + stat;
-    put(b > CAP ? 0 : T, b);
+static void deriv(const drmb200_topology_t* topo, bool fold, bool prefolded, bool fd) {
+    g_rnea_fold = fold ? 1 : 0;
+    FoldChoice fc;
+    const int rc = select_fold(topo, prefolded, &fc);
+    if (rc != DRMB200_OK) { put(rc, 0); return; }
+    if (fc.prog->n_dofs == 0) { put(-1000, 0); return; }        // nothing to launch
+    const bool staging_fold = fc.fold.n_red > 0 && fc.fold.n_full > 0;
+    put(deriv_tile(*fc.prog, staging_fold ? fc.fold.n_full : 0, fd, STATIC_DERIV), STATIC_DERIV);
 }
 
 int main() {
@@ -84,39 +76,24 @@ int main() {
         }
         topo.n_dofs = n_dofs;
 
-        int rc_cp = 0, rc = 0;
-        const CachedPrograms* cp = cached_programs(&topo, &rc_cp);
-        for (int k = 0; k < 6; ++k) {
-            if (cp == nullptr) { put(rc_cp, 0); continue; }
-            deriv(cp, k < 2, k >= 4, k & 1);
-        }
+        for (int k = 0; k < 6; ++k) deriv(&topo, k < 2, k >= 4, k & 1);
 
         PathProgram path;
-        rc = build_path_program(&topo, links[0], &path);
+        int rc = build_path_program(&topo, links[0], &path);
         if (rc != DRMB200_OK) put(rc, 0);
-        else {
-            auto bytes_of = [&](int T) { return (size_t)IkSmemLayout(T, path.n_dofs, path.len).total_floats * 4 + STATIC_IK; };
-            const int T = bytes_of(64) <= TWO_CTAS ? 64 : 32;
-            put(bytes_of(T) > CAP ? 0 : T, bytes_of(T));
-        }
+        else put(ik_tile(path, STATIC_IK), STATIC_IK);
 
-        MultiProgram W;
-        rc = build_multi_program(&topo, n_ee, links, &W);
-        int n_u = 0;
-        if (rc == DRMB200_OK)
-            for (int k = 0; k < W.n_steps; ++k) n_u += W.dof[k] >= 0;
+        UnionProgram P;
+        rc = build_union_program(&topo, n_ee, links, &P);
         for (int pose = 1; pose >= 0; --pose) {
-            if (rc != DRMB200_OK) { put(rc, 0); continue; }
-            ladder([&](int T) { return IkmSmemLayout(T, W.n_dofs, n_u, n_ee, pose, W.n_steps, W.n_jslots, W.n_state_slots).total_floats; },
-                   STATIC_IKM);
+            if (rc != DRMB200_OK) put(rc, 0);
+            else put(ikm_tile(P, pose, STATIC_IKM), STATIC_IKM);
         }
+        int rc_cp = 0;
+        const CachedPrograms* cp = cached_programs(&topo, &rc_cp);
         for (int pose = 1; pose >= 0; --pose) {
-            if (rc != DRMB200_OK || cp == nullptr) { put(rc != DRMB200_OK ? rc : rc_cp, 0); continue; }
-            OsdProgram P;
-            P.walk = W;
-            P.n_u = n_u;
-            const int M = (pose ? 6 : 3) * n_ee;
-            ladder([&](int T) { return OsdSmemLayout(T, cp->full, P, M).total_floats; }, STATIC_OSD);
+            if (rc != DRMB200_OK || cp == nullptr) put(rc != DRMB200_OK ? rc : rc_cp, 0);
+            else put(osd_tile(cp->full, P, (pose ? 6 : 3) * n_ee, STATIC_OSD), STATIC_OSD);
         }
         std::printf("\n");
         ++count;

@@ -373,8 +373,8 @@ def test_static_shared_memory_is_what_the_mirrors_add():
     symbols = {"deriv": ["_ZN3drm27dynamics_derivatives_kernelILb0EEEvNS_11TreeProgramENS_11FoldProgramENS_9DerivArgsE",
                          "_ZN3drm27dynamics_derivatives_kernelILb1EEEvNS_11TreeProgramENS_11FoldProgramENS_9DerivArgsE"],
                "ik": [f"_ZN3drm25inverse_kinematics_kernelILb{b}EEEvNS_11PathProgramENS_6IkArgsE" for b in (0, 1)],
-               "ikm": [f"_ZN3drm31inverse_kinematics_multi_kernelILb{b}EEEvNS_10IkmProgramENS_7IkmArgsE" for b in (0, 1)],
-               "osd": [f"_ZN3drm24operational_space_kernelILi{t}EEEvNS_11TreeProgramENS_10OsdProgramENS_7OsdArgsE"
+               "ikm": [f"_ZN3drm31inverse_kinematics_multi_kernelILb{b}EEEvNS_12UnionProgramENS_7IkmArgsE" for b in (0, 1)],
+               "osd": [f"_ZN3drm24operational_space_kernelILi{t}EEEvNS_11TreeProgramENS_12UnionProgramENS_7OsdArgsE"
                        for t in TM.LADDER]}
     for kernel, syms in symbols.items():
         for sym in syms:

@@ -1,11 +1,10 @@
 """Python mirrors of the host-side tile choosers of four kernels, and of the shared-memory layouts they size tiles by:
 
-  * dynamics_derivatives.cu  launch_derivatives: TC = 128 / n configurations per CTA, lowered one by one while the CTA
+  * dynamics_derivatives.cu  deriv_tile: TC = 128 / n configurations per CTA, lowered one by one while the CTA
                              (DerivSmemLayout) exceeds 113 KB; ELIMIT when TC = 1 still exceeds 227 KB;
-  * inverse_kinematics.cu    launch_ik: T = 64 rows per CTA if IkSmemLayout(64) fits 113 KB, else 32;
-  * inverse_kinematics_multi.cu  launch_ikm: T = 64, 32, ..., 1 (IkmSmemLayout), first that fits 113 KB;
-  * operational_space.cu     operational_space_dynamics_device: the same ladder over OsdSmemLayout (one template
-                             instantiation per rung).
+  * inverse_kinematics.cu    ik_tile: T = 64 rows per CTA if IkSmemLayout(64) fits 113 KB, else 32;
+  * inverse_kinematics_multi.cu  ikm_tile: T = 64, 32, ..., 1 (IkmSmemLayout), first that fits 113 KB;
+  * operational_space.cu     osd_tile: the same ladder over OsdSmemLayout (one template instantiation per rung).
 
 Every chooser adds the kernel's static shared memory (STATIC_SMEM, what `-Xptxas -v` reports) to the dynamic bytes.
 tests/host_checks/tile_check.cu evaluates the real layout structs on the real programs; tests/test_tile_choice.py pins
@@ -43,7 +42,7 @@ def deriv_floats(tc, n, n_links, n_slots, fold_full, fd):
 
 
 def deriv_choice(n, n_links, n_slots, fold_full, fd) -> Choice:
-    """launch_derivatives' tile for a program of n_links links (n movable) and n_slots branch slots; fold_full is the
+    """deriv_tile's tile for a program of n_links links (n movable) and n_slots branch slots; fold_full is the
     full link count when the kernel folds while staging, else 0."""
     static = STATIC_SMEM["deriv"]
     tc = 1 if n >= 128 else 128 // n
