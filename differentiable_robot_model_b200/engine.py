@@ -103,6 +103,8 @@ _SIGNATURES = {
                                                           ctypes.POINTER(ctypes.c_int32), _c_float_p, _c_float_p, _c_float_p,
                                                           _c_float_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_int32,
                                                           _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
+    "drmb200_dynamics_regressor": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                  ctypes.c_int64, ctypes.c_uint32, _c_float_p, ctypes.c_void_p]),
     "drmb200_kinematic_state": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
                                                _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table": (ctypes.c_int, [_c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_void_p]),
@@ -346,6 +348,20 @@ def forward_dynamics_derivatives_raw(topo, table, q, qd, f, flags, folded=None, 
                                                             flags & 3, *[_ptr(o) for o in outs], _stream())
     _check(rc, "drmb200_forward_dynamics_derivatives")
     return tuple(outs)
+
+
+def dynamics_regressor_raw(topo, table, q, qd, qdd, flags, out=None):
+    """Y [B, n, n_links, 14], Y[b, i, l, k] = d tau_i / d table[l, 12 + k], so that einsum("bilk,lk->bi", Y, table[:, 12:26])
+    is the inverse dynamics of the same inputs; one launch (drmb200_dynamics_regressor, always on the unfolded table)."""
+    _require_cuda(table, q, qd, qdd, out)
+    q, qd, qdd = q.contiguous(), qd.contiguous(), qdd.contiguous()
+    B, n = q.shape
+    Y = out if out is not None else torch.empty((B, n, topo.n_links, 14), device=q.device, dtype=torch.float32)
+    with _on(q.device):
+        rc = lib().drmb200_dynamics_regressor(ctypes.byref(topo), _ptr(table.contiguous()), _ptr(q), _ptr(qd), _ptr(qdd), B,
+                                              flags & 3, _ptr(Y), _stream())
+    _check(rc, "drmb200_dynamics_regressor")
+    return Y
 
 
 def forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags, want_qdd=True):

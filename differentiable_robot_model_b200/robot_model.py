@@ -478,6 +478,48 @@ class DifferentiableRobotModel(torch.nn.Module):
         return engine.forward_dynamics_derivatives_raw(self._topology, table, q.detach(), qd.detach(), f.detach(), flags,
                                                        folded=self._folded_table())
 
+    @tensor_check
+    def compute_dynamics_regressor(
+        self,
+        q: torch.Tensor,
+        qd: torch.Tensor,
+        qdd_des: torch.Tensor,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = True,
+    ) -> torch.Tensor:
+        r"""The joint-torque regressor of the inertial parameters in ONE launch (``csrc/dynamics_regressor.cu``).
+
+        Args:
+            q, qd, qdd_des: joint angles / velocities / desired accelerations [batch_size x n_dofs]
+            include_gravity, use_damping: as for :meth:`compute_inverse_dynamics`
+        Returns: ``Y`` [batch_size x n_dofs x n_links x 14] (``[n_dofs x n_links x 14]`` for 1-D inputs) with
+        ``Y[b, i, l, k] = d tau_i / d pi[l, k]``, ``pi = inertial_parameters()``, so that
+        ``einsum("bilk,lk->bi", Y, pi)`` is :meth:`compute_inverse_dynamics` of the same inputs.  The output carries no
+        autograd graph: it uses the current values of the link parameters (learnable and fused ones included) and, being
+        linear in them, does not depend on the inertial ones at all."""
+        self._check_q(q, qd, qdd_des)
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table().detach()
+        return engine.dynamics_regressor_raw(self._topology, table, q.detach(), qd.detach(), qdd_des.detach(), flags)
+
+    def inertial_parameters(self) -> torch.Tensor:
+        r"""Every link's inertial parameters and damping, ``[n_links x 14]`` in URDF link order (the root first): the link
+        table's columns 12:26,
+
+            ``I_o`` (9, row-major) | ``m c`` (3) | ``m`` | joint damping,
+
+        with ``I_o = I_c + m S(c) S(c)^T`` the rotational inertia about the link frame's origin.  Differentiable when link
+        parameters are learnable.  For every configuration
+
+            ``einsum("bilk,lk->bi", compute_dynamics_regressor(q, qd, qdd), inertial_parameters())
+            == compute_inverse_dynamics(q, qd, qdd)``
+
+        (same ``include_gravity`` / ``use_damping``).  ``I_o`` is not symmetrised, so its nine entries are nine columns of
+        the regressor.  The standard symmetric 10-parameter form per link, ``(Ixx, Ixy, Ixz, Iyy, Iyz, Izz, mcx, mcy, mcz,
+        m)``, has the regressor columns of ``I_o[a, a]`` and, for ``a != b``, the sum of the ``I_o[a, b]`` and ``I_o[b, a]``
+        columns."""
+        return self._link_table()[:, 12:26]
+
     def compute_operational_space_dynamics(
         self,
         q: torch.Tensor,

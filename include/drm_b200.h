@@ -27,6 +27,8 @@
  *   drmb200_inverse_kinematics_multi     the same for several links at once (one solve over their stacked errors).
  *   drmb200_operational_space_dynamics   inverse operational-space inertia J G J^T and the velocities, bias and true
  *                                        accelerations of several links, one launch (the reference has none of these).
+ *   drmb200_dynamics_regressor           the joint-torque regressor Y, tau = Y . (I_o, mc, m, damping of every link), one
+ *                                        launch (the reference: autograd of compute_inverse_dynamics, row by row).
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -402,6 +404,29 @@ int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n
                                        int64_t batch, uint32_t flags, int32_t position_only, float* inv_inertia,
                                        float* acceleration, float* velocity, float* bias_acceleration,
                                        void* cuda_stream);
+
+/*
+ * The joint-torque regressor of the inertial parameters and dampings, one launch (csrc/dynamics_regressor.cu).  tau is
+ * linear in every link's table entries 12:26 (I_o 9 row-major | mc 3 | m | damping), so for any table
+ *   tau_i(q, qd, qdd) = sum_{l, k} Y[b, i, l, k] * table[l, 12 + k]         (Y . pi = tau)
+ * where tau is exactly what drmb200_inverse_dynamics computes with the same table, flags and inputs.
+ *   Y [B, n_dofs, n_links, 14], fp32, row-major:  Y[b, i, l, k] = d tau_i / d table[l, 12 + k], columns in the table's
+ *     order; the entries of I_o are independent columns (non-symmetric I_o included: adding the I_o[a][b] and I_o[b][a]
+ *     columns gives the usual symmetric 10-parameter form).  Every link has its own 14 columns: a fixed link's parameters
+ *     reach tau through its movable ancestor, so its columns are not zero.  Exact zeros: the root's columns, the columns of
+ *     links outside the subtree of dof i's link, the damping column of fixed links and, without DRMB200_DAMPING, every
+ *     damping column.  With DRMB200_DAMPING, Y[b, dof(l), l, 13] = qd[b, dof(l)].  DRMB200_GRAVITY enters through the base
+ *     acceleration, as in RNEA.
+ * The regressor needs a column per table row, so it always walks the full (unfolded) tree: there is no _prefolded variant
+ * and the "rnea_fold" option does not affect it.  Inputs: q, qd, qdd [B, n_dofs], table; device pointers, a
+ * caller-allocated output that must not alias the inputs.  No allocation, no synchronisation (graph-capturable).
+ * batch == 0 and models without movable joints are a no-op.  DRMB200_EINVAL for a null pointer or a negative batch;
+ * DRMB200_ELIMIT for more live branch points than the tree program holds (as drmb200_inverse_dynamics) and, naming the
+ * bytes needed, when one configuration per CTA needs more than 227 KB of shared memory (56 n_dofs n_links B of output each).
+ */
+int drmb200_dynamics_regressor(const drmb200_topology_t* topo, const float* table,
+                               const float* q, const float* qd, const float* qdd,
+                               int64_t batch, uint32_t flags, float* Y, void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state
