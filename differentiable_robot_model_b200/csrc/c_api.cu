@@ -116,6 +116,8 @@ int operational_space_dynamics_device(const drmb200_topology_t*, int32_t, const 
                                       const float*, int64_t, uint32_t, int32_t, float*, float*, float*, float*, cudaStream_t);
 int dynamics_regressor_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t, uint32_t,
                               float*, cudaStream_t);
+int energy_momentum_device(const drmb200_topology_t*, const float*, const float*, const float*, int64_t, float*, float*, float*,
+                           float*, float*, float*, cudaStream_t);
 int64_t table_grad_workspace_bytes(const drmb200_topology_t*, int64_t);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 int mass_matrix_device(const drmb200_topology_t*, const float*, const float*, int64_t, float*, cudaStream_t);
@@ -451,6 +453,13 @@ int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n
 int drmb200_dynamics_regressor(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                                const float* qdd, int64_t batch, uint32_t flags, float* Y, void* cuda_stream) {
     return drm::dynamics_regressor_device(topo, table, q, qd, qdd, batch, flags, Y, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_energy_momentum(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd, int64_t batch,
+                            float* kinetic, float* potential, float* momentum, float* com, float* com_velocity,
+                            float* com_jacobian, void* cuda_stream) {
+    return drm::energy_momentum_device(topo, table, q, qd, batch, kinetic, potential, momentum, com, com_velocity, com_jacobian,
+                                       static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_kinematic_state(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

@@ -201,15 +201,6 @@ __device__ __forceinline__ void aba_unit_response(const TreeProgram& prog, const
     }
 }
 
-// slot-major shared tile [e][T] -> contiguous global block [valid][per_row]
-__device__ __forceinline__ void store_transposed(float* dst, const float* src, int per_row, int valid, int T) {
-    const int total = valid * per_row;
-    for (int i = threadIdx.x; i < total; i += blockDim.x) {
-        const int r = i / per_row, e = i - r * per_row;
-        dst[i] = src[e * T + r];
-    }
-}
-
 template <int T>
 __global__ void __launch_bounds__(T)
 operational_space_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ UnionProgram P, const OsdArgs args) {

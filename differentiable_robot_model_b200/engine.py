@@ -105,6 +105,9 @@ _SIGNATURES = {
                                                           _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_dynamics_regressor": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                   ctypes.c_int64, ctypes.c_uint32, _c_float_p, ctypes.c_void_p]),
+    "drmb200_energy_momentum": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
+                                               _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                               ctypes.c_void_p]),
     "drmb200_kinematic_state": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
                                                _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table": (ctypes.c_int, [_c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_void_p]),
@@ -362,6 +365,28 @@ def dynamics_regressor_raw(topo, table, q, qd, qdd, flags, out=None):
                                               flags & 3, _ptr(Y), _stream())
     _check(rc, "drmb200_dynamics_regressor")
     return Y
+
+
+def energy_momentum_raw(topo, table, q, qd=None, want_kinetic=True, want_potential=True, want_momentum=True, want_com=True,
+                        want_com_velocity=True, want_com_jacobian=True):
+    """(kinetic [B], potential [B], momentum [B, n], com [B, 3], com_velocity [B, 3], com_jacobian [B, 3, n]), one launch
+    (drmb200_energy_momentum, always on the unfolded table).  An output not wanted is None; without qd the velocity-dependent
+    ones (kinetic, momentum, com_velocity) are None as well."""
+    _require_cuda(table, q, qd)
+    q = q.contiguous()
+    qd = None if qd is None else qd.contiguous()
+    B, n = q.shape
+    dev = q.device
+    has_qd = qd is not None
+    shapes = ((B,), (B,), (B, n), (B, 3), (B, 3), (B, 3, n))
+    wants = (want_kinetic and has_qd, want_potential, want_momentum and has_qd, want_com, want_com_velocity and has_qd,
+             want_com_jacobian)
+    outs = [torch.empty(s, device=dev, dtype=torch.float32) if w else None for s, w in zip(shapes, wants)]
+    with _on(dev):
+        rc = lib().drmb200_energy_momentum(ctypes.byref(topo), _ptr(table.contiguous()), _ptr(q), _ptr(qd), B,
+                                           *[_ptr(o) for o in outs], _stream())
+    _check(rc, "drmb200_energy_momentum")
+    return tuple(outs)
 
 
 def forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags, want_qdd=True):

@@ -104,6 +104,18 @@ class OperationalSpaceDynamics(NamedTuple):
     bias_acceleration: torch.Tensor
 
 
+class EnergyAndMomentum(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_energy_and_momentum` returns, per row: the kinetic and potential energy
+    [J], the generalized momentum ``H(q) qd`` [n_dofs], the centre of mass [3] and its velocity [3] in the world frame, and
+    the CoM Jacobian [3 x n_dofs].  The three velocity-dependent fields are None when no ``qd`` was given."""
+    kinetic_energy: Optional[torch.Tensor]
+    potential_energy: torch.Tensor
+    momentum: Optional[torch.Tensor]
+    com: torch.Tensor
+    com_velocity: Optional[torch.Tensor]
+    com_jacobian: torch.Tensor
+
+
 class DifferentiableRobotModel(torch.nn.Module):
     """Batched rigid-body kinematics / dynamics of a URDF robot on one GPU (H100, sm_90a)."""
 
@@ -519,6 +531,34 @@ class DifferentiableRobotModel(torch.nn.Module):
         m)``, has the regressor columns of ``I_o[a, a]`` and, for ``a != b``, the sum of the ``I_o[a, b]`` and ``I_o[b, a]``
         columns."""
         return self._link_table()[:, 12:26]
+
+    def compute_energy_and_momentum(self, q: torch.Tensor, qd: Optional[torch.Tensor] = None) -> EnergyAndMomentum:
+        r"""Whole-body quantities of every configuration in ONE launch (``csrc/energy_momentum.cu``; the definitions are
+        stated in ``include/drm_b200.h``): kinetic energy ``1/2 sum_i <V_i, I_i V_i>``, potential energy in gravity
+        ``(0, 0, -9.81)`` (zero at z = 0), generalized momentum, centre of mass ``com`` (zeros for a massless model), its
+        world-frame velocity and its Jacobian.  For every configuration, up to rounding,
+            ``momentum = H qd`` with ``H = compute_lagrangian_inertia_matrix(q)``,
+            ``kinetic_energy = 1/2 qd . momentum``,
+            ``d potential_energy / dq = compute_inverse_dynamics(q, 0, 0, include_gravity=True, use_damping=False)
+            = 9.81 M com_jacobian[2]`` (M the total mass),
+            ``com_jacobian = d com / dq`` and ``com_velocity = com_jacobian qd``.
+
+        Args:
+            q: joint angles [batch_size x n_dofs]
+            qd: joint velocities [batch_size x n_dofs], or None: ``kinetic_energy``, ``momentum`` and ``com_velocity`` are
+                then None (the other fields are bit-identical to a call with qd)
+        Returns: :class:`EnergyAndMomentum` with shapes [batch_size], [batch_size], [batch_size x n_dofs], [batch_size x 3],
+        [batch_size x 3], [batch_size x 3 x n_dofs], squeezed for 1-D inputs.  The outputs carry no autograd graph: they use
+        the current values of the link parameters (learnable and fused ones included) but are not differentiable."""
+        return EnergyAndMomentum(*self._energy_and_momentum(q, qd))
+
+    @tensor_check
+    def _energy_and_momentum(self, q, qd):
+        given = [t for t in (q, qd) if t is not None]
+        self._check_q(*given)
+        assert all(t.dtype == torch.float32 for t in given), "the engine is fp32-only"
+        table = self._link_table().detach()
+        return engine.energy_momentum_raw(self._topology, table, q.detach(), None if qd is None else qd.detach())
 
     def compute_operational_space_dynamics(
         self,

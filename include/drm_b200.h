@@ -29,6 +29,8 @@
  *                                        accelerations of several links, one launch (the reference has none of these).
  *   drmb200_dynamics_regressor           the joint-torque regressor Y, tau = Y . (I_o, mc, m, damping of every link), one
  *                                        launch (the reference: autograd of compute_inverse_dynamics, row by row).
+ *   drmb200_energy_momentum              kinetic and potential energy, generalized momentum H(q) qd, centre of mass, its
+ *                                        velocity and its Jacobian, one launch (the reference has none of these).
  *   drmb200_fk_jacobian_host   the same FK+Jacobian op on HOST buffers (pinned or pageable):
  *                              chunked H2D -> kernel -> D2H pipeline on internal streams.
  *
@@ -427,6 +429,37 @@ int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n
 int drmb200_dynamics_regressor(const drmb200_topology_t* topo, const float* table,
                                const float* q, const float* qd, const float* qdd,
                                int64_t batch, uint32_t flags, float* Y, void* cuda_stream);
+
+/*
+ * Whole-body quantities of a configuration, one launch (csrc/energy_momentum.cu).  They hold for any link table: learnable,
+ * fused and non-symmetric I_o included.  For every link i, root included:
+ *   (R_i, p_i) is its world pose and (w_i, v_i) its body-frame spatial velocity, exactly as drmb200_kinematic_state returns
+ *   them; m_i = table[i, 24], mc_i = table[i, 21:24] and I_o,i = table[i, 12:21] (row-major, not symmetrised); M = sum_i m_i.
+ *   For a movable link j, z_j is its world joint axis and p_j its origin, as in the Jacobian; sub(j) is link j and its
+ *   descendants.  (f_lin, f_ang) = I_i V_i = (m v - mc x w, I_o w + mc x v), the reference's multiply_motion_vec.
+ * Outputs, caller-allocated, fp32, row-major:
+ *   kinetic       [B]        sum_i 1/2 m_i |v_i|^2 + 1/2 w_i^T I_o,i w_i + v_i . (w_i x mc_i)  (= 1/2 sum_i <V_i, I_i V_i>)
+ *   potential     [B]        9.81 sum_i (m_i p_i,z + (R_i mc_i)_z): gravity is (0, 0, -9.81), the same as the DRMB200_GRAVITY
+ *                            base acceleration; zero at z = 0
+ *   momentum      [B, n]     momentum[dof(j)] = z_j . sum_{i in sub(j)} (R_i f_ang,i + (p_i - p_j) x R_i f_lin,i).  This equals
+ *                            H(q) qd for the H of drmb200_mass_matrix, for any table
+ *   com           [B, 3]     sum_i (m_i p_i + R_i mc_i) / M
+ *   com_velocity  [B, 3]     sum_i R_i (m_i v_i + w_i x mc_i) / M, world frame
+ *   com_jacobian  [B, 3, n]  column dof(j) = z_j x (sum_{i in sub(j)} (m_i p_i + R_i mc_i) - (sum_{i in sub(j)} m_i) p_j) / M,
+ *                            so com_velocity = com_jacobian qd; a joint whose subtree is massless gets an exactly zero column
+ * If M == 0 exactly, com, com_velocity and com_jacobian are written as zeros, not NaN.  kinetic = 1/2 qd . momentum holds
+ * mathematically; only the symmetric part of I_o enters kinetic.
+ * NULL skips an output (all NULL: nothing is launched).  qd [B, n_dofs] may be NULL only when kinetic, momentum and
+ * com_velocity are all NULL; the other outputs do not depend on it and are bit-identical either way.  It always walks the
+ * full (unfolded) tree: there is no _prefolded variant and "rnea_fold" does not affect it.  Inputs: q [B, n_dofs], table;
+ * device pointers, outputs must not alias inputs.  No allocation, no synchronisation (graph-capturable).  batch == 0 is a
+ * no-op.  DRMB200_EINVAL for a null table or q, a null qd that is needed, or a negative batch; DRMB200_ELIMIT for more
+ * live branch points than the tree program holds and, naming the bytes, when a one-row CTA needs more than 227 KB of shared
+ * memory (about 16 n_links + 4 n_dofs floats per row: no model within DRMB200_MAX_LINKS reaches it).
+ */
+int drmb200_energy_momentum(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
+                            int64_t batch, float* kinetic, float* potential, float* momentum, float* com,
+                            float* com_velocity, float* com_jacobian, void* cuda_stream);
 
 /*
  * World pose (and body-frame spatial velocity) of EVERY link in one launch: replaces update_kinematic_state
