@@ -127,8 +127,8 @@ int kinematic_state_device(const drmb200_topology_t*, const float*, const float*
 int build_table_backward_device(const float*, const float*, int32_t, float*, cudaStream_t);
 int build_table_fused_device(const float*, const float*, const int32_t*, const int32_t*, const float*, int32_t, float*, float*,
                              cudaStream_t);
-int build_table_fused_backward_device(const float*, const float*, const float*, const int32_t*, const int32_t*, int32_t, int32_t,
-                                      float*, float*, cudaStream_t);
+int build_table_fused_backward_device(const float*, const float*, const float*, const int32_t*, const int32_t*, const int32_t*,
+                                      int32_t, int32_t, float*, float*, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------------
 // host-buffer pipeline for FK + Jacobian
@@ -482,11 +482,12 @@ int drmb200_build_link_table_fused(const float* const_raw, const float* flat, co
                                          static_cast<cudaStream_t>(cuda_stream));
 }
 
-int drmb200_build_link_table_fused_backward(const float* raw, const float* table_grad, const float* flat, const int32_t* src,
-                                            const int32_t* kind, int32_t n_links, int32_t n_flat, float* raw_grad_scratch,
-                                            float* flat_grad, void* cuda_stream) {
-    return drm::build_table_fused_backward_device(raw, table_grad, flat, src, kind, n_links, n_flat, raw_grad_scratch, flat_grad,
-                                                  static_cast<cudaStream_t>(cuda_stream));
+int drmb200_build_link_table_fused_backward(const float* raw, const float* table_grad, const float* flat,
+                                            const int32_t* first_reader, const int32_t* next_reader, const int32_t* kind,
+                                            int32_t n_links, int32_t n_flat, float* raw_grad_scratch, float* flat_grad,
+                                            void* cuda_stream) {
+    return drm::build_table_fused_backward_device(raw, table_grad, flat, first_reader, next_reader, kind, n_links, n_flat,
+                                                  raw_grad_scratch, flat_grad, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_fk_jacobian_host(const drmb200_topology_t* topo, int32_t ee_link, int32_t device, const float* table,

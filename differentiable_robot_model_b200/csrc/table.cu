@@ -128,16 +128,18 @@ __global__ void build_table_fused_kernel(const float* __restrict__ const_raw, co
     t[24] = m; t[25] = r[19]; t[26] = 0.f; t[27] = 0.f;
 }
 
-// raw_grad (as build_table_backward_kernel) scattered into the gradient of the flat vector; entries of `flat` that feed
-// nothing (modules on fixed-joint origins, which the reference freezes) get zero
-__global__ void scatter_flat_grad_kernel(const float* __restrict__ g_raw, const float* __restrict__ flat,
-                                         const int32_t* __restrict__ src, const int32_t* __restrict__ kind, int n_raw,
-                                         int n_flat, float* __restrict__ g_flat) {
-    for (int k = threadIdx.x; k < n_flat; k += blockDim.x) g_flat[k] = 0.f;
-    __syncthreads();
-    for (int k = threadIdx.x; k < n_raw; k += blockDim.x) {
-        const int sidx = src[k];
-        if (sidx >= 0) g_flat[sidx] = kind[k] == 1 ? 2.f * flat[sidx] * g_raw[k] : g_raw[k];
+// raw_grad (as build_table_backward_kernel) gathered into the gradient of the flat vector.  One thread per flat entry sums
+// the raw entries that read it -- the list first_reader[s], next_reader[.], ... (-1 ends it), ascending raw indices -- in
+// that order: a parameter tied across several links gets the sum of their gradients, and the sum is bitwise repeatable
+// (no atomics).  Entries of `flat` nothing reads (modules on fixed-joint origins, which the reference freezes) get zero.
+__global__ void gather_flat_grad_kernel(const float* __restrict__ g_raw, const float* __restrict__ flat,
+                                        const int32_t* __restrict__ first_reader, const int32_t* __restrict__ next_reader,
+                                        const int32_t* __restrict__ kind, int n_flat, float* __restrict__ g_flat) {
+    for (int s = threadIdx.x; s < n_flat; s += blockDim.x) {
+        const float p2 = 2.f * flat[s];
+        float g = 0.f;
+        for (int k = first_reader[s]; k >= 0; k = next_reader[k]) g += kind[k] == 1 ? p2 * g_raw[k] : g_raw[k];
+        g_flat[s] = g;
     }
 }
 
@@ -169,13 +171,13 @@ int build_table_fused_device(const float* const_raw, const float* flat, const in
     return DRMB200_OK;
 }
 
-int build_table_fused_backward_device(const float* raw, const float* g_table, const float* flat, const int32_t* src,
-                                      const int32_t* kind, int32_t n_links, int32_t n_flat, float* g_raw_scratch,
-                                      float* g_flat, cudaStream_t stream) {
+int build_table_fused_backward_device(const float* raw, const float* g_table, const float* flat, const int32_t* first_reader,
+                                      const int32_t* next_reader, const int32_t* kind, int32_t n_links, int32_t n_flat,
+                                      float* g_raw_scratch, float* g_flat, cudaStream_t stream) {
     if (n_links < 1 || n_links > DRMB200_MAX_LINKS) { set_error("n_links=%d outside [1, %d]", n_links, DRMB200_MAX_LINKS); return DRMB200_ELIMIT; }
-    if (raw == nullptr || g_table == nullptr || flat == nullptr || src == nullptr || kind == nullptr || g_raw_scratch == nullptr || g_flat == nullptr || n_flat < 0) { set_error("null pointer argument"); return DRMB200_EINVAL; }
+    if (raw == nullptr || g_table == nullptr || flat == nullptr || first_reader == nullptr || next_reader == nullptr || kind == nullptr || g_raw_scratch == nullptr || g_flat == nullptr || n_flat < 0) { set_error("null pointer argument"); return DRMB200_EINVAL; }
     build_table_backward_kernel<<<1, 64, 0, stream>>>(raw, g_table, n_links, g_raw_scratch);
-    scatter_flat_grad_kernel<<<1, 256, 0, stream>>>(g_raw_scratch, flat, src, kind, n_links * RAW_STRIDE, n_flat, g_flat);
+    gather_flat_grad_kernel<<<1, 256, 0, stream>>>(g_raw_scratch, flat, first_reader, next_reader, kind, n_flat, g_flat);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("build_table_fused_backward launch: %s", cudaGetErrorString(e)); return DRMB200_ECUDA; }
     count_launch(2);

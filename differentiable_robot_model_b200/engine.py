@@ -116,8 +116,8 @@ _SIGNATURES = {
     "drmb200_build_link_table_fused": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, _c_float_p,
                                                       ctypes.c_int32, _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_build_link_table_fused_backward": (ctypes.c_int, [_c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
-                                                               ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, _c_float_p,
-                                                               _c_float_p, ctypes.c_void_p]),
+                                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                               _c_float_p, _c_float_p, ctypes.c_void_p]),
     "drmb200_comm_create": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(ctypes.c_void_p),
                                            ctypes.c_void_p]),
     "drmb200_comm_connect": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
@@ -586,10 +586,11 @@ class BuildLinkTableFunction(torch.autograd.Function):
 class FusedTableFunction(torch.autograd.Function):
     """flat link-parameter vector [P] -> link table [n_links, 28] in ONE launch (drmb200_build_link_table_fused): the
     per-(link, parameter) parametrisation modules are applied inside the kernel through an index / kind / offset map.
-    Backward: table_grad -> flat_grad, two tiny launches.  One leaf, one AccumulateGrad node, one optimiser tensor."""
+    Backward: table_grad -> flat_grad, two tiny launches; a flat entry read by several raw entries (a tied parameter) gets
+    the sum of their gradients in a fixed order.  One leaf, one AccumulateGrad node, one optimiser tensor."""
 
     @staticmethod
-    def forward(ctx, flat, const_raw, src, kind, off):
+    def forward(ctx, flat, const_raw, src, kind, off, first_reader, next_reader):
         _require_cuda(flat, const_raw, off)
         flat = flat.contiguous()
         n_links = const_raw.shape[0]
@@ -599,22 +600,22 @@ class FusedTableFunction(torch.autograd.Function):
             rc = lib().drmb200_build_link_table_fused(_ptr(const_raw), _ptr(flat), _ptr(src), _ptr(kind), _ptr(off), n_links,
                                                       _ptr(raw), _ptr(table), _stream())
         _check(rc, "drmb200_build_link_table_fused")
-        ctx.save_for_backward(flat, raw, src, kind)
+        ctx.save_for_backward(flat, raw, kind, first_reader, next_reader)
         return table
 
     @staticmethod
     def backward(ctx, g_table):
-        flat, raw, src, kind = ctx.saved_tensors
+        flat, raw, kind, first_reader, next_reader = ctx.saved_tensors
         g_table = g_table.contiguous()
         _require_cuda(g_table)
         g_flat = torch.empty_like(flat)
         scratch = torch.empty_like(raw)
         with _on(flat.device):
-            rc = lib().drmb200_build_link_table_fused_backward(_ptr(raw), _ptr(g_table), _ptr(flat), _ptr(src), _ptr(kind),
-                                                               raw.shape[0], flat.numel(), _ptr(scratch), _ptr(g_flat),
-                                                               _stream())
+            rc = lib().drmb200_build_link_table_fused_backward(_ptr(raw), _ptr(g_table), _ptr(flat), _ptr(first_reader),
+                                                               _ptr(next_reader), _ptr(kind), raw.shape[0], flat.numel(),
+                                                               _ptr(scratch), _ptr(g_flat), _stream())
         _check(rc, "drmb200_build_link_table_fused_backward")
-        return g_flat, None, None, None, None
+        return g_flat, None, None, None, None, None, None
 
 
 class FkJacobianFunction(torch.autograd.Function):

@@ -155,7 +155,14 @@ class FusedLinkParameters(torch.nn.Module):
     ``PositiveScalar`` (``l^2 + min_val``) -- the ones the reference's examples use
     (``examples/learn_dynamics_iiwa.py:57-65``); anything else raises and the model stays on the per-module path.
     The modules' own Parameters are re-pointed at slices of the flat storage, so ``print_learnable_params`` /
-    ``state_dict`` keep showing the live values; only the flat vector receives gradients."""
+    ``state_dict`` keep showing the live values; only the flat vector receives gradients.
+
+    * Tied parameters: a module installed on several links owns ONE slice of ``flat`` that every one of its raw entries
+      reads; its gradient is the sum over those entries, as autograd gives on the per-module path.  So
+      ``flat.numel()`` is the number of parameter values that required grad before fusing.
+    * Frozen modules (no parameter requires grad when fusing, ``freeze_learnable_link_param``): their current output is
+      written into the constant block and they stay out of ``flat`` -- no gradient, no optimiser update, whatever the
+      optimiser does with zero gradients.  The value is fixed from then on; freezing is decided before fusing."""
 
     def __init__(self, bodies, device):
         super().__init__()
@@ -165,30 +172,39 @@ class FusedLinkParameters(torch.nn.Module):
         src = torch.full((n_raw,), -1, dtype=torch.int32)
         kind = torch.zeros(n_raw, dtype=torch.int32)
         off = torch.zeros(n_raw, dtype=torch.float32)
-        chunks, owners, cursor = [], [], 0
+        chunks, owners, cursor = [], {}, 0                # owners: id(param) -> (param, start of its slice of flat)
 
-        def claim(param, raw_offset, size, k, o, module):
+        def claim(param, size, module):
             nonlocal cursor
             if param.numel() != size:
                 raise ValueError(f"{type(module).__name__}: {param.numel()} values for a link parameter of {size}")
-            chunks.append(param.detach().reshape(-1).to(dtype=torch.float32, device=device))
-            owners.append((param, cursor))
-            if raw_offset is not None:
-                src[raw_offset:raw_offset + size] = torch.arange(cursor, cursor + size, dtype=torch.int32)
-                kind[raw_offset:raw_offset + size] = k
-                off[raw_offset:raw_offset + size] = o
-            cursor += size
+            if id(param) not in owners:                   # a tied module is claimed once, by its first link
+                chunks.append(param.detach().reshape(-1).to(dtype=torch.float32, device=device))
+                owners[id(param)] = (param, cursor)
+                cursor += size
+            return owners[id(param)][1]
+
+        def frozen(module):
+            return not any(p_.requires_grad for p_ in module.parameters())
 
         seen = set()
         for module, raw_offset, size in learnable:
+            seen.add(id(module))
+            if frozen(module):
+                with torch.no_grad():
+                    const[raw_offset:raw_offset + size] = module().reshape(size).to(dtype=torch.float32, device=device)
+                continue
             if isinstance(module, PositiveScalar):
-                claim(module.l, raw_offset, size, 1, float(module._min_val), module)
+                param, k, o = module.l, 1, float(module._min_val)
             elif isinstance(module, (UnconstrainedScalar, UnconstrainedTensor)):
-                claim(module.param, raw_offset, size, 0, 0.0, module)
+                param, k, o = module.param, 0, 0.0
             else:
                 raise ValueError(f"cannot fuse a {type(module).__name__} parametrisation (supported: UnconstrainedScalar, "
                                  "UnconstrainedTensor, PositiveScalar); the model keeps evaluating its modules one by one")
-            seen.add(id(module))
+            start = claim(param, size, module)
+            src[raw_offset:raw_offset + size] = torch.arange(start, start + size, dtype=torch.int32)
+            kind[raw_offset:raw_offset + size] = k
+            off[raw_offset:raw_offset + size] = o
         # modules on fixed-joint origins feed nothing (reference quirk, rigid_body.py:64-67) but stay parameters
         for body in bodies:
             for owner, names in ((body, ("trans", "rot_angles", "joint_damping")), (body.inertia, ("mass", "com", "inertia_mat"))):
@@ -196,19 +212,31 @@ class FusedLinkParameters(torch.nn.Module):
                     module = getattr(owner, name)
                     if isinstance(module, torch.nn.Module) and id(module) not in seen:
                         for p_ in module.parameters():
-                            claim(p_, None, p_.numel(), 0, 0.0, module)
+                            if p_.requires_grad:
+                                claim(p_, p_.numel(), module)
+        # the inverse of src for the backward: per flat entry, the list of the raw entries that read it, ascending
+        first_reader = torch.full((cursor,), -1, dtype=torch.int32)
+        next_reader = torch.full((n_raw,), -1, dtype=torch.int32)
+        for k in reversed(torch.nonzero(src >= 0).flatten().tolist()):
+            next_reader[k] = first_reader[src[k]]
+            first_reader[src[k]] = k
+        # does `flat` feed a joint origin (rpy | trans of a movable link)?  If not, kinematics need no parameter gradient
+        self.feeds_kinematics = bool((src.reshape(-1, RAW_STRIDE)[:, :6] >= 0).any())
         self.flat = torch.nn.Parameter(torch.cat(chunks) if chunks else torch.zeros(0, device=device))
         self.register_buffer("const_raw", const.reshape(len(bodies), RAW_STRIDE).contiguous(), persistent=False)
         self.register_buffer("src", src.to(device), persistent=False)
         self.register_buffer("kind", kind.to(device), persistent=False)
         self.register_buffer("off", off.to(device), persistent=False)
-        for param, start in owners:                       # the modules' Parameters become views of the flat storage
+        self.register_buffer("first_reader", first_reader.to(device), persistent=False)
+        self.register_buffer("next_reader", next_reader.to(device), persistent=False)
+        for param, start in owners.values():             # the modules' Parameters become views of the flat storage
             param.data = self.flat.data[start:start + param.numel()].view(param.shape)
             param.requires_grad_(False)                   # gradients (and optimiser updates) go through `flat` only
 
     def table(self):
         from . import engine
-        return engine.FusedTableFunction.apply(self.flat, self.const_raw, self.src, self.kind, self.off)
+        return engine.FusedTableFunction.apply(self.flat, self.const_raw, self.src, self.kind, self.off, self.first_reader,
+                                               self.next_reader)
 
 
 def build_link_table(bodies, device):

@@ -230,12 +230,22 @@ class DifferentiableRobotModel(torch.nn.Module):
         """Gather every learnable link parameter into ONE flat ``nn.Parameter`` (returned; also
         ``model.fused_link_params.flat``): the link table is then built from it by one kernel, the backward leaves one
         gradient tensor and ``torch.optim.Adam(model.parameters(), fused=True)`` updates everything in one launch.  Call
-        after the last ``make_link_param_learnable``; values and gradients are the same as on the per-module path (the
-        modules' own Parameters become views of the flat storage and stop requiring grad).  Raises ``ValueError`` for
-        parametrisations other than UnconstrainedScalar / UnconstrainedTensor / PositiveScalar."""
+        once, after the last ``make_link_param_learnable``; values and gradients are the same as on the per-module path
+        (the modules' own Parameters become views of the flat storage and stop requiring grad):
+
+        * a module installed on several links (tied parameters) owns one slice of the flat vector and receives the sum
+          of the gradients of all its links;
+        * a module that is frozen (``freeze_learnable_link_param``) when this is called stays out of the flat vector:
+          its current value becomes a constant of the table, so it gets no gradient and no optimiser can move it.
+          Freezing is decided before fusing -- afterwards ``freeze_`` / ``unfreeze_learnable_link_param``,
+          ``make_link_param_learnable`` and a second ``fuse_learnable_parameters`` raise ``RuntimeError``.
+
+        Raises ``ValueError`` for (unfrozen) parametrisations other than UnconstrainedScalar / UnconstrainedTensor /
+        PositiveScalar; the model then stays on the per-module path."""
         if self._device.type != "cuda":
             raise RuntimeError("fuse_learnable_parameters needs a CUDA model")
-        self.fused_link_params = None
+        if getattr(self, "fused_link_params", None) is not None:
+            raise RuntimeError("fuse_learnable_parameters() called twice: the model is already fused")
         self.fused_link_params = FusedLinkParameters(self._bodies, self._device)
         return self.fused_link_params.flat
 
@@ -243,6 +253,9 @@ class DifferentiableRobotModel(torch.nn.Module):
         """True if any joint origin (``trans`` / ``rot_angles`` of a movable link) is a learnable module with a
         parameter that requires grad -- then the backward kernels must produce the F / r columns of the table
         gradient; otherwise the RNEA backward can take the single-sweep inertial path."""
+        fused = getattr(self, "fused_link_params", None)
+        if fused is not None:                                  # the flat vector carries everything that can learn
+            return fused.feeds_kinematics and fused.flat.requires_grad
         for body in self._bodies:
             if body.joint_idx is None:
                 continue
@@ -250,11 +263,6 @@ class DifferentiableRobotModel(torch.nn.Module):
                 attr = getattr(body, name)
                 if isinstance(attr, torch.nn.Module):
                     params = list(attr.parameters())
-                    fused = getattr(self, "fused_link_params", None)
-                    if fused is not None and params:                            # views of the flat vector
-                        if fused.flat.requires_grad:
-                            return True
-                        continue
                     if not params or any(p.requires_grad for p in params):      # parameter-free modules: be safe
                         return True
         return False
@@ -898,13 +906,23 @@ class DifferentiableRobotModel(torch.nn.Module):
         assert isinstance(module, torch.nn.Module), f"{parameter_name} of {link_name} is not a learnable module."
         return module
 
+    def _set_learnable_link_param_frozen(self, link_name: str, parameter_name: str, frozen: bool):
+        module = self._learnable_module(link_name, parameter_name)
+        if getattr(self, "fused_link_params", None) is not None:
+            raise RuntimeError("freeze / unfreeze_learnable_link_param after fuse_learnable_parameters(): the flat vector "
+                               "holds what was unfrozen when it was built; freeze before fusing")
+        for param in module.parameters():
+            param.requires_grad = not frozen
+
     def freeze_learnable_link_param(self, link_name: str, parameter_name: str):
-        for param in self._learnable_module(link_name, parameter_name).parameters():
-            param.requires_grad = False
+        """Stop learning this link parameter: its module keeps its value and gets no gradient.  A module installed on
+        several links is frozen on all of them.  Call before ``fuse_learnable_parameters`` (raises ``RuntimeError``
+        after): a frozen module's value becomes a constant of the fused table."""
+        self._set_learnable_link_param_frozen(link_name, parameter_name, True)
 
     def unfreeze_learnable_link_param(self, link_name: str, parameter_name: str):
-        for param in self._learnable_module(link_name, parameter_name).parameters():
-            param.requires_grad = True
+        """Undo ``freeze_learnable_link_param`` (raises ``RuntimeError`` after ``fuse_learnable_parameters``)."""
+        self._set_learnable_link_param_frozen(link_name, parameter_name, False)
 
     # ------------------------------------------------------------------------------------------
     # introspection (robot_model.py:715-754)

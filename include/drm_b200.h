@@ -490,15 +490,20 @@ int drmb200_build_link_table_backward(const float* raw, const float* table_grad,
  * Fused parametrisation (BASELINE config 5): every learnable entry of the raw block is a function of ONE flat device vector,
  *   raw[k] = const_raw[k] (src[k] < 0) | flat[src[k]] (kind[k] == 0) | flat[src[k]]^2 + off[k] (kind[k] == 1),
  * which covers the reference's UnconstrainedScalar / UnconstrainedTensor / PositiveScalar modules
- * (rigid_body_params.py:14-56).  Forward: one launch (raw rows are written to raw_out for the backward, then the table as
- * above).  Backward: table_grad -> flat_grad [n_flat] (two tiny launches; raw_grad_scratch [n_links, 20] is workspace).
+ * (rigid_body_params.py:14-56).  Several raw entries may read one flat entry (a parameter tied across links).
+ * Forward: one launch (raw rows are written to raw_out for the backward, then the table as above).
+ * Backward: table_grad -> flat_grad [n_flat] (two tiny launches; raw_grad_scratch [n_links, 20] is workspace).  The
+ * inverse of src is passed as linked lists: first_reader[s] (n_flat entries) is the lowest raw index k with src[k] == s and
+ * next_reader[k] (n_links * DRMB200_RAW_STRIDE entries) the next higher one, -1 for none; flat_grad[s] is the sum over that
+ * list in that order, so it is bitwise repeatable, and zero for an entry nothing reads.
  * All pointers are device pointers; src / kind / off have n_links * DRMB200_RAW_STRIDE entries.
  */
 int drmb200_build_link_table_fused(const float* const_raw, const float* flat, const int32_t* src, const int32_t* kind,
                                    const float* off, int32_t n_links, float* raw_out, float* table, void* cuda_stream);
 int drmb200_build_link_table_fused_backward(const float* raw, const float* table_grad, const float* flat,
-                                            const int32_t* src, const int32_t* kind, int32_t n_links, int32_t n_flat,
-                                            float* raw_grad_scratch, float* flat_grad, void* cuda_stream);
+                                            const int32_t* first_reader, const int32_t* next_reader, const int32_t* kind,
+                                            int32_t n_links, int32_t n_flat, float* raw_grad_scratch, float* flat_grad,
+                                            void* cuda_stream);
 
 /*
  * Host-buffer variant of drmb200_fk_jacobian: q and the outputs are HOST pointers (pinned memory

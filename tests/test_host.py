@@ -286,6 +286,80 @@ def test_fused_parameter_map_reproduces_the_per_module_raw_rows():
     assert all(not p.requires_grad for n, p in m.named_parameters())
 
 
+def _fused_raw(fused):
+    """The (src, kind, off) map of a FusedLinkParameters applied to its flat vector on the CPU -> raw rows."""
+    flat, src = fused.flat.detach(), fused.src.long()
+    vals = torch.where(fused.kind == 1, flat[src.clamp_min(0)] ** 2 + fused.off, flat[src.clamp_min(0)])
+    return torch.where(src >= 0, vals, fused.const_raw.reshape(-1)).reshape(fused.const_raw.shape)
+
+
+def test_fused_layout_gives_a_tied_module_one_slice_and_lists_all_its_readers():
+    """One module installed on several links is ONE parameter: the fused layout gives it one slice of the flat vector
+    that every one of its raw entries reads, and the reader lists the backward kernel sums over (first_reader /
+    next_reader, the inverse of src) name each of those entries once, in ascending order."""
+    from differentiable_robot_model_b200.link_table import RAW_STRIDE, FusedLinkParameters, gather_raw_parameters
+    from differentiable_robot_model_b200.rigid_body_params import PositiveScalar
+    torch.manual_seed(0)
+    m = drm.DifferentiableKUKAiiwa(device="cpu")
+    mass, com = PositiveScalar(min_val=0.25), UnconstrainedTensor(dim1=1, dim2=3)
+    for link in ("iiwa_link_1", "iiwa_link_2"):
+        m.make_link_param_learnable(link, "mass", mass)
+        m.make_link_param_learnable(link, "com", com)
+    n_values = sum(p.numel() for p in m.parameters())
+    assert n_values == 4
+    want = gather_raw_parameters(m._bodies, torch.device("cpu")).detach().clone()
+    fused = FusedLinkParameters(m._bodies, torch.device("cpu"))
+    assert fused.flat.numel() == n_values
+    assert torch.equal(_fused_raw(fused), want)
+    src = fused.src.reshape(-1, RAW_STRIDE)
+    assert torch.equal(src[1, 6:10], src[2, 6:10]) and int((src >= 0).sum()) == 8
+    # every flat entry's reader list names exactly the raw entries whose src is that entry, ascending
+    first, nxt = fused.first_reader.tolist(), fused.next_reader.tolist()
+    assert len(first) == n_values and len(nxt) == fused.src.numel()
+    for s in range(n_values):
+        readers, k = [], first[s]
+        while k >= 0:
+            readers.append(k)
+            k = nxt[k]
+        assert readers == torch.nonzero(fused.src == s).flatten().tolist() and len(readers) == 2
+    # both links follow the one slice, and the module's own Parameter is a view of it
+    with torch.no_grad():
+        fused.flat.mul_(1.5)
+    raw = _fused_raw(fused)
+    assert torch.equal(raw[1, 6:10], raw[2, 6:10]) and not torch.equal(raw[1, 6:10], want[1, 6:10])
+    assert mass.l.data_ptr() in (fused.flat.data_ptr() + 4 * k for k in range(n_values))
+    assert float(mass()) == float(raw[1, 6])
+
+
+def test_fused_layout_keeps_a_frozen_module_out_of_the_flat_vector():
+    """A module frozen before fusing is a constant of the fused table: its value sits in the constant block, no entry of the
+    flat vector feeds it, and its Parameter stays its own storage -- so no optimiser step on the flat vector can move it."""
+    from differentiable_robot_model_b200.link_table import RAW_STRIDE, FusedLinkParameters, gather_raw_parameters
+    from differentiable_robot_model_b200.rigid_body_params import PositiveScalar
+    torch.manual_seed(0)
+    m = drm.DifferentiableKUKAiiwa(device="cpu")
+    m.make_link_param_learnable("iiwa_link_1", "mass", PositiveScalar(min_val=0.5))
+    m.make_link_param_learnable("iiwa_link_2", "trans", UnconstrainedTensor(dim1=1, dim2=3))
+    m.make_link_param_learnable("iiwa_link_3", "com", UnconstrainedTensor(dim1=1, dim2=3))
+    m.make_link_param_learnable("iiwa_link_ee", "trans", UnconstrainedTensor(dim1=1, dim2=3))      # fixed joint, frozen too
+    for link, name in (("iiwa_link_1", "mass"), ("iiwa_link_2", "trans"), ("iiwa_link_ee", "trans")):
+        m.freeze_learnable_link_param(link, name)
+    want = gather_raw_parameters(m._bodies, torch.device("cpu")).detach().clone()
+    fused = FusedLinkParameters(m._bodies, torch.device("cpu"))
+    assert fused.flat.numel() == 3                               # the com alone
+    src = fused.src.reshape(-1, RAW_STRIDE)
+    assert int((src >= 0).sum()) == 3 and bool((src[3, 7:10] >= 0).all())
+    assert not fused.feeds_kinematics                            # the only joint origin that was learnable is frozen
+    assert torch.equal(_fused_raw(fused), want)
+    with torch.no_grad():
+        fused.flat.add_(1.0)
+    raw = _fused_raw(fused)
+    assert torch.equal(raw[1], want[1]) and torch.equal(raw[2], want[2]) and not torch.equal(raw[3], want[3])
+    lo, hi = fused.flat.data_ptr(), fused.flat.data_ptr() + 4 * fused.flat.numel()
+    for frozen in (m._bodies[1].inertia.mass.l, m._bodies[2].trans.param, m._bodies[8].trans.param):
+        assert not lo <= frozen.data_ptr() < hi and not frozen.requires_grad
+
+
 def test_tuning_options_round_trip_without_a_gpu():
     """drmb200_set_option / drmb200_get_option are host-side state: defaults, round trip, unknown names."""
     from differentiable_robot_model_b200 import engine
