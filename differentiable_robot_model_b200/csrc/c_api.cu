@@ -114,6 +114,10 @@ int inverse_kinematics_multi_device(const drmb200_topology_t*, int32_t, const in
                                     float*, float*, float*, uint8_t*, float*, cudaStream_t);
 int operational_space_dynamics_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
                                       const float*, int64_t, uint32_t, int32_t, float*, float*, float*, float*, cudaStream_t);
+int contact_dynamics_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                            const float*, const float*, int64_t, uint32_t, int32_t, float, float*, float*, uint8_t*, cudaStream_t);
+int contact_impulse_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                           const float*, int64_t, int32_t, float, float*, float*, uint8_t*, cudaStream_t);
 int dynamics_regressor_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t, uint32_t,
                               float*, cudaStream_t);
 int energy_momentum_device(const drmb200_topology_t*, const float*, const float*, const float*, int64_t, float*, float*, float*,
@@ -448,6 +452,21 @@ int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n
     return drm::operational_space_dynamics_device(topo, n_ee, ee_links, table, q, qd, f, batch, flags, position_only, inv_inertia,
                                                   acceleration, velocity, bias_acceleration,
                                                   static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_contact_dynamics(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                             const float* q, const float* qd, const float* f, const float* accel_ref, int64_t batch,
+                             uint32_t flags, int32_t position_only, float regularization, float* qdd, float* force,
+                             uint8_t* solved, void* cuda_stream) {
+    return drm::contact_dynamics_device(topo, n_ee, ee_links, table, q, qd, f, accel_ref, batch, flags, position_only,
+                                        regularization, qdd, force, solved, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_contact_impulse(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                            const float* q, const float* qd, const float* velocity_ref, int64_t batch, int32_t position_only,
+                            float regularization, float* qd_plus, float* impulse, uint8_t* solved, void* cuda_stream) {
+    return drm::contact_impulse_device(topo, n_ee, ee_links, table, q, qd, velocity_ref, batch, position_only, regularization,
+                                       qd_plus, impulse, solved, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_dynamics_regressor(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

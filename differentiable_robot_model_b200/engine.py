@@ -103,6 +103,13 @@ _SIGNATURES = {
                                                           ctypes.POINTER(ctypes.c_int32), _c_float_p, _c_float_p, _c_float_p,
                                                           _c_float_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_int32,
                                                           _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
+    "drmb200_contact_dynamics": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                                _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
+                                                ctypes.c_uint32, ctypes.c_int32, ctypes.c_float, _c_float_p, _c_float_p,
+                                                ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_contact_impulse": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                               _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int32,
+                                               ctypes.c_float, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
     "drmb200_dynamics_regressor": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                   ctypes.c_int64, ctypes.c_uint32, _c_float_p, ctypes.c_void_p]),
     "drmb200_energy_momentum": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
@@ -490,6 +497,59 @@ def operational_space_dynamics_raw(topo, ee_links, table, q, qd, f, flags, posit
                                                       *[_ptr(v) for v in vecs], _stream())
     _check(rc, "drmb200_operational_space_dynamics")
     return (inv, *vecs)
+
+
+CONTACT_PIVOT_MIN = 1e-5     # compiled into csrc/contact_dynamics.cu: smallest pivot of the equilibrated system that solves
+
+
+def contact_dynamics_raw(topo, ee_links, table, q, qd, f, flags, accel_ref=None, position_only=False, regularization=0.0,
+                         want_force=True):
+    """(qdd [B, n], force [B, M] or None, solved [B] bool) of rigid contacts at the links `ee_links`, M = 6 len(ee_links)
+    (3 with position_only), one launch (drmb200_contact_dynamics).  accel_ref [B, M] or None (0)."""
+    _require_cuda(table, q, qd, f, accel_ref)
+    q, qd, f = q.contiguous(), qd.contiguous(), f.contiguous()
+    accel_ref = None if accel_ref is None else accel_ref.contiguous()
+    B, n = q.shape
+    E = len(ee_links)
+    M = (3 if position_only else 6) * E
+    if accel_ref is not None and tuple(accel_ref.shape) != (B, M):
+        raise RuntimeError(f"accel_ref: expected shape {(B, M)}, got {tuple(accel_ref.shape)}")
+    dev = q.device
+    qdd = torch.empty((B, n), device=dev, dtype=torch.float32)
+    force = torch.empty((B, M), device=dev, dtype=torch.float32) if want_force else None
+    solved = torch.empty(B, device=dev, dtype=torch.uint8)
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    with _on(dev):
+        rc = lib().drmb200_contact_dynamics(ctypes.byref(topo), E, links, _ptr(table), _ptr(q), _ptr(qd), _ptr(f),
+                                            _ptr(accel_ref), B, flags & 3, 1 if position_only else 0,
+                                            ctypes.c_float(regularization), _ptr(qdd), _ptr(force), _ptr(solved), _stream())
+    _check(rc, "drmb200_contact_dynamics")
+    return qdd, force, solved.view(torch.bool)
+
+
+def contact_impulse_raw(topo, ee_links, table, q, qd, velocity_ref=None, position_only=False, regularization=0.0,
+                        want_impulse=True):
+    """(qd_plus [B, n], impulse [B, M] or None, solved [B] bool) of an impact at the links `ee_links`, M = 6 len(ee_links)
+    (3 with position_only), one launch (drmb200_contact_impulse).  velocity_ref [B, M] or None (0: inelastic)."""
+    _require_cuda(table, q, qd, velocity_ref)
+    q, qd = q.contiguous(), qd.contiguous()
+    velocity_ref = None if velocity_ref is None else velocity_ref.contiguous()
+    B, n = q.shape
+    E = len(ee_links)
+    M = (3 if position_only else 6) * E
+    if velocity_ref is not None and tuple(velocity_ref.shape) != (B, M):
+        raise RuntimeError(f"velocity_ref: expected shape {(B, M)}, got {tuple(velocity_ref.shape)}")
+    dev = q.device
+    qd_plus = torch.empty((B, n), device=dev, dtype=torch.float32)
+    impulse = torch.empty((B, M), device=dev, dtype=torch.float32) if want_impulse else None
+    solved = torch.empty(B, device=dev, dtype=torch.uint8)
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    with _on(dev):
+        rc = lib().drmb200_contact_impulse(ctypes.byref(topo), E, links, _ptr(table), _ptr(q), _ptr(qd), _ptr(velocity_ref), B,
+                                           1 if position_only else 0, ctypes.c_float(regularization), _ptr(qd_plus),
+                                           _ptr(impulse), _ptr(solved), _stream())
+    _check(rc, "drmb200_contact_impulse")
+    return qd_plus, impulse, solved.view(torch.bool)
 
 
 def kinematic_state_raw(topo, table, q, qd=None, want_poses=True, want_quats=False):

@@ -104,6 +104,25 @@ class OperationalSpaceDynamics(NamedTuple):
     bias_acceleration: torch.Tensor
 
 
+class ContactDynamics(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_contact_dynamics` returns, per row: the joint accelerations under the
+    contacts [n_dofs], the contact forces ``lambda`` [M] (world frame, at each link origin; 6 per link, force over torque, or
+    3 for position only, links stacked in the order requested) and whether the row's contact system was solved (bool; an
+    unsolved row has NaN in both)."""
+    qdd: torch.Tensor
+    force: torch.Tensor
+    solved: torch.Tensor
+
+
+class ContactImpulse(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_contact_impulse` returns, per row: the joint velocities just after the
+    impact [n_dofs], the contact impulses ``Lambda`` [M] (laid out like :class:`ContactDynamics`'s force) and whether the
+    row's contact system was solved."""
+    qd_plus: torch.Tensor
+    impulse: torch.Tensor
+    solved: torch.Tensor
+
+
 class EnergyAndMomentum(NamedTuple):
     """What :meth:`DifferentiableRobotModel.compute_energy_and_momentum` returns, per row: the kinetic and potential energy
     [J], the generalized momentum ``H(q) qd`` [n_dofs], the centre of mass [3] and its velocity [3] in the world frame, and
@@ -611,6 +630,100 @@ class DifferentiableRobotModel(torch.nn.Module):
         table = self._link_table().detach()
         return engine.operational_space_dynamics_raw(self._topology, links, table, q.detach(), qd.detach(), f.detach(), flags,
                                                      position_only=bool(position_only))
+
+    def compute_contact_dynamics(
+        self,
+        q: torch.Tensor,
+        qd: torch.Tensor,
+        f: torch.Tensor,
+        link_names: List[str],
+        accel_ref: Optional[torch.Tensor] = None,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = False,
+        position_only: bool = False,
+        regularization: float = 0.0,
+    ) -> ContactDynamics:
+        r"""Forward dynamics with the links held by bilateral rigid contacts (at most 8, distinct), in ONE launch
+        (``csrc/contact_dynamics.cu``; the definition and the solve are stated in ``include/drm_b200.h``).  With ``J``, ``G``,
+        ``qdd_free`` and ``Jdot qd`` as in :meth:`compute_operational_space_dynamics` and ``mu = regularization``:
+
+        * ``A = J G J^T + mu I`` and ``lambda`` solves ``A lambda = accel_ref - (J qdd_free + Jdot qd)``;
+        * ``qdd = qdd_free + G J^T lambda``, which is :meth:`compute_forward_dynamics` at ``f + J^T lambda``;
+        * ``force = lambda``: the world-frame force (and torque, in pose mode) applied at each link origin;
+        * hence ``J qdd + Jdot qd = accel_ref - mu lambda``: the links move with the requested acceleration when ``mu = 0``.
+          For symmetric inertias this is Gauss's principle, ``H (qdd - qdd_free) = J^T lambda``.
+
+        Args:
+            q, qd, f: joint angles / velocities / applied joint forces [batch_size x n_dofs]
+            link_names: the held links, stacked in this order; each needs a movable joint on its root path
+            accel_ref: the desired constraint-space acceleration [batch_size x M] (e.g. Baumgarte terms); None: 0
+            include_gravity, use_damping: as for :meth:`compute_forward_dynamics`
+            position_only: hold the link origins only (3 rows per link) instead of the full pose (6)
+            regularization: ``mu >= 0``; redundant constraint sets (more rows than the joints can satisfy) need ``mu > 0``
+        Returns: :class:`ContactDynamics` ``(qdd, force, solved)``, squeezed for 1-D inputs.  A row whose equilibrated system
+        has a pivot of magnitude <= 1e-5 is not solved: ``solved`` is False and its outputs are NaN.  The outputs carry no
+        autograd graph: they use the current values of the link parameters (learnable and fused ones included) but are not
+        differentiable."""
+        links = self._contact_links(link_names)
+        out = self._contact_dynamics(q, qd, f, accel_ref, links=links, include_gravity=include_gravity,
+                                     use_damping=use_damping, position_only=bool(position_only),
+                                     regularization=float(regularization))
+        return ContactDynamics(*out)
+
+    def compute_contact_impulse(
+        self,
+        q: torch.Tensor,
+        qd: torch.Tensor,
+        link_names: List[str],
+        velocity_ref: Optional[torch.Tensor] = None,
+        position_only: bool = False,
+        regularization: float = 0.0,
+    ) -> ContactImpulse:
+        r"""The joint velocities after an instantaneous impact at the links (at most 8, distinct), in ONE launch
+        (``csrc/contact_dynamics.cu``; stated in ``include/drm_b200.h``).  With ``J`` and ``G`` as in
+        :meth:`compute_operational_space_dynamics` and ``mu = regularization``:
+
+        * ``Lambda`` solves ``(J G J^T + mu I) Lambda = velocity_ref - J qd``;
+        * ``qd_plus = qd + G J^T Lambda`` and ``impulse = Lambda``, so ``J qd_plus = velocity_ref - mu Lambda``.
+
+        Gravity, damping and applied forces do not act during the impulse.  ``velocity_ref = None`` (0) is a perfectly
+        inelastic impact, which does not increase the kinetic energy; ``velocity_ref = -e J qd`` is restitution ``e``, and
+        ``e = 1`` with ``mu = 0`` keeps the kinetic energy (symmetric inertias).
+
+        Args:
+            q, qd: joint angles / velocities before the impact [batch_size x n_dofs]
+            link_names, position_only, regularization: as for :meth:`compute_contact_dynamics`
+            velocity_ref: the desired constraint-space velocity after the impact [batch_size x M]; None: 0
+        Returns: :class:`ContactImpulse` ``(qd_plus, impulse, solved)``, squeezed for 1-D inputs; unsolved rows as in
+        :meth:`compute_contact_dynamics`.  No autograd graph, current link parameters."""
+        links = self._contact_links(link_names)
+        out = self._contact_impulse(q, qd, velocity_ref, links=links, position_only=bool(position_only),
+                                    regularization=float(regularization))
+        return ContactImpulse(*out)
+
+    def _contact_links(self, link_names):
+        links = [self._name_to_idx_map[name] for name in link_names]      # KeyError for unknown links
+        assert len(set(links)) == len(links), "link names must be distinct"
+        return links
+
+    @tensor_check
+    def _contact_dynamics(self, q, qd, f, accel_ref, links, include_gravity, use_damping, position_only, regularization):
+        self._check_q(q, qd, f)
+        M = (3 if position_only else 6) * len(links)
+        assert accel_ref is None or tuple(accel_ref.shape) == (q.shape[0], M), f"accel_ref must be [batch_size x {M}]"
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table().detach()
+        return engine.contact_dynamics_raw(self._topology, links, table, q.detach(), qd.detach(), f.detach(), flags,
+                                           None if accel_ref is None else accel_ref.detach(), position_only, regularization)
+
+    @tensor_check
+    def _contact_impulse(self, q, qd, velocity_ref, links, position_only, regularization):
+        self._check_q(q, qd)
+        M = (3 if position_only else 6) * len(links)
+        assert velocity_ref is None or tuple(velocity_ref.shape) == (q.shape[0], M), f"velocity_ref must be [batch_size x {M}]"
+        table = self._link_table().detach()
+        return engine.contact_impulse_raw(self._topology, links, table, q.detach(), qd.detach(),
+                                          None if velocity_ref is None else velocity_ref.detach(), position_only, regularization)
 
     def compute_inverse_kinematics(
         self,

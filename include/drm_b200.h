@@ -27,6 +27,9 @@
  *   drmb200_inverse_kinematics_multi     the same for several links at once (one solve over their stacked errors).
  *   drmb200_operational_space_dynamics   inverse operational-space inertia J G J^T and the velocities, bias and true
  *                                        accelerations of several links, one launch (the reference has none of these).
+ *   drmb200_contact_dynamics / drmb200_contact_impulse   joint accelerations and contact forces under rigid contacts at
+ *                                        several links, and the joint velocities and impulses of an impact there, one launch
+ *                                        each (the reference has none of these).
  *   drmb200_dynamics_regressor           the joint-torque regressor Y, tau = Y . (I_o, mc, m, damping of every link), one
  *                                        launch (the reference: autograd of compute_inverse_dynamics, row by row).
  *   drmb200_energy_momentum              kinetic and potential energy, generalized momentum H(q) qd, centre of mass, its
@@ -406,6 +409,55 @@ int drmb200_operational_space_dynamics(const drmb200_topology_t* topo, int32_t n
                                        int64_t batch, uint32_t flags, int32_t position_only, float* inv_inertia,
                                        float* acceleration, float* velocity, float* bias_acceleration,
                                        void* cuda_stream);
+
+/*
+ * Contact dynamics and contact impulses of bilateral rigid contacts at SEVERAL links, one launch each
+ * (csrc/contact_dynamics.cu).  Per row b, for the model, the distinct links ee_links [n_ee] (host array, 1 <= n_ee <= 8),
+ * position_only and a regularisation mu = `regularization` >= 0:
+ *   J [M, n_dofs]  the stacked geometric Jacobians exactly as drmb200_operational_space_dynamics builds them (link frame
+ *                  origin, world frame, 3 linear rows over 3 angular rows, M = 6 n_ee; only the linear rows, M = 3 n_ee, with
+ *                  position_only != 0).
+ *   G [n, n]       the same dqdd_df as there: the articulated-body algorithm at (q, 0, e_j) without gravity or damping; H^-1
+ *                  for a symmetric inertia, the articulated-body arithmetic for a non-symmetric inertia_mat.
+ *   A [M, M]       J G J^T + mu I_M: the operational-space inv_inertia plus mu on the diagonal.
+ * Contact dynamics (drmb200_contact_dynamics), with the call's flags (DRMB200_GRAVITY, DRMB200_DAMPING):
+ *   b        = J qdd_free + Jdot qd, qdd_free = forward dynamics at (q, qd, f): the operational-space `acceleration`;
+ *   lambda   solves A lambda = a_ref - b, a_ref [B, M] the desired constraint-space acceleration (accel_ref; NULL: 0);
+ *   qdd      [B, n]  qdd_free + G J^T lambda (= forward dynamics at (q, qd, f + J^T lambda): the ABA is affine in f);
+ *   force    [B, M]  lambda: the stacked world-frame force applied at each link origin (and torque, in pose mode), the
+ *                    convention of the operational-space acceleration(f + J^T F).
+ *   Hence J qdd + Jdot qd = a_ref - mu lambda.
+ * Contact impulse (drmb200_contact_impulse), no flags and no f: gravity, damping and applied forces do not act during an
+ * instantaneous impulse:
+ *   Lambda   solves A Lambda = v_ref - J qd, v_ref [B, M] the desired post-impact constraint velocity (velocity_ref; NULL:
+ *            0, a perfectly inelastic impact; restitution e is v_ref = -e J qd);
+ *   qd_plus  [B, n]  qd + G J^T Lambda;
+ *   impulse  [B, M]  Lambda.
+ *   Hence J qd_plus = v_ref - mu Lambda.
+ * The solve: Jacobi equilibration s_k = |A_kk|^-1/2, then Gaussian elimination with partial pivoting on S A S (ties go to
+ * the lower row index) and back substitution; the solution is S y.  A row is UNSOLVED when some A_kk is zero or not finite
+ * or when a pivot of S A S is not finite or has magnitude <= 1e-5 (CONTACT_PIVOT_MIN, compiled in): it gets solved[b] = 0
+ * and NaN in both outputs; a solved row gets solved[b] = 1.  The equilibration makes the threshold independent of units:
+ * pose rows mix m/s^2 per N with rad/s^2 per N m.  Redundant constraint sets (more independent rows than the joints can
+ * satisfy, e.g. 4 pose fingertips on iiwa7_allegro, M = 24 > 23 joints, or the planar 2-link arm in pose mode) are
+ * unsolved at mu = 0 and need mu > 0.
+ * Outputs, caller-allocated, fp32 / uint8, row-major, must not alias inputs; force / impulse may be NULL (skipped), qdd /
+ * qd_plus and solved are required.  Inputs: q, qd, f [B, n_dofs], table; device pointers.  No allocation, no
+ * synchronisation (graph-capturable).  batch == 0 is a no-op (no launch).  DRMB200_EINVAL for n_ee outside [1, 8], a link
+ * index out of range, a link given twice, a link with no movable joint on its root path (the root included: its rows are
+ * zero and never solvable), a negative or non-finite regularization, a null required pointer (batch > 0: empty tensors may
+ * have null data) or a negative batch;
+ * DRMB200_ELIMIT for more live branch points than the forward-dynamics kernel handles or, naming the bytes, when a one-row
+ * CTA needs more than 227 KB of shared memory.
+ */
+int drmb200_contact_dynamics(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                             const float* q, const float* qd, const float* f, const float* accel_ref, int64_t batch,
+                             uint32_t flags, int32_t position_only, float regularization,
+                             float* qdd, float* force, uint8_t* solved, void* cuda_stream);
+int drmb200_contact_impulse(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                            const float* q, const float* qd, const float* velocity_ref, int64_t batch,
+                            int32_t position_only, float regularization,
+                            float* qd_plus, float* impulse, uint8_t* solved, void* cuda_stream);
 
 /*
  * The joint-torque regressor of the inertial parameters and dampings, one launch (csrc/dynamics_regressor.cu).  tau is
