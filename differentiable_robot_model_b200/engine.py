@@ -615,31 +615,66 @@ def _workspace(topo, batch, device):
 # ------------------------------------------------------------------------------------------------
 # autograd
 # ------------------------------------------------------------------------------------------------
+SECOND_ORDER_UNSUPPORTED = (
+    "second-order derivatives through the engine's kernels are not supported: the analytic backward kernels are "
+    "first-order only (their gradients carry no graph of their own). Differentiate the kinematic Jacobian outputs "
+    "(compute_endeffector_jacobian / compute_fk_and_jacobian) or use compute_inverse_dynamics_derivatives / "
+    "compute_forward_dynamics_derivatives instead.")
+
+
+class _FirstOrderOnly(torch.autograd.Function):
+    """Identity on a gradient returned by a kernel backward under ``create_graph=True``.  Its inputs include the primals
+    of that backward and its upstream gradients, so the result requires grad and sits on the path from them; its backward
+    raises.  Without it torch treats the kernel's gradient as a constant, and a Hessian or a gradient penalty silently
+    gets zeros where the second-order term should be."""
+
+    @staticmethod
+    def forward(ctx, grad, *depends_on):
+        return grad.view_as(grad)
+
+    @staticmethod
+    def backward(ctx, *_):
+        raise RuntimeError(SECOND_ORDER_UNSUPPORTED)
+
+
+def first_order_only(grads, depends_on):
+    """``grads`` (a tuple, None entries allowed) unchanged outside ``create_graph``; under it (grad mode on inside a
+    backward), each gradient wrapped so that differentiating it raises, provided any tensor of ``depends_on`` requires
+    grad -- otherwise no second-order path exists and nothing is wrapped."""
+    if not torch.is_grad_enabled():
+        return grads
+    deps = [t for t in depends_on if isinstance(t, torch.Tensor) and t.requires_grad]
+    if not deps:
+        return grads
+    return tuple(g if g is None else _FirstOrderOnly.apply(g, *deps) for g in grads)
+
+
 class BuildLinkTableFunction(torch.autograd.Function):
     """raw link parameters [n_links, 20] -> link table [n_links, 28] (csrc/table.cu), one launch each way."""
 
     @staticmethod
     def forward(ctx, raw):
         _require_cuda(raw)
+        ctx.save_for_backward(raw)
         raw = raw.contiguous()
         n_links = raw.shape[0]
         table = torch.empty((n_links, 28), device=raw.device, dtype=torch.float32)
         with _on(raw.device):
             rc = lib().drmb200_build_link_table(_ptr(raw), n_links, _ptr(table), _stream())
         _check(rc, "drmb200_build_link_table")
-        ctx.save_for_backward(raw)
         return table
 
     @staticmethod
     def backward(ctx, g_table):
-        (raw,) = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        raw = saved[0].contiguous()
         g_table = g_table.contiguous()
         _require_cuda(g_table)
         g_raw = torch.empty_like(raw)
         with _on(raw.device):
             rc = lib().drmb200_build_link_table_backward(_ptr(raw), _ptr(g_table), raw.shape[0], _ptr(g_raw), _stream())
         _check(rc, "drmb200_build_link_table_backward")
-        return g_raw
+        return first_order_only((g_raw,), saved + (g_table,))[0]
 
 
 
@@ -652,6 +687,7 @@ class FusedTableFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, flat, const_raw, src, kind, off, first_reader, next_reader):
         _require_cuda(flat, const_raw, off)
+        flat_in = flat
         flat = flat.contiguous()
         n_links = const_raw.shape[0]
         raw = torch.empty_like(const_raw)
@@ -660,12 +696,13 @@ class FusedTableFunction(torch.autograd.Function):
             rc = lib().drmb200_build_link_table_fused(_ptr(const_raw), _ptr(flat), _ptr(src), _ptr(kind), _ptr(off), n_links,
                                                       _ptr(raw), _ptr(table), _stream())
         _check(rc, "drmb200_build_link_table_fused")
-        ctx.save_for_backward(flat, raw, kind, first_reader, next_reader)
+        ctx.save_for_backward(flat_in, raw, kind, first_reader, next_reader)
         return table
 
     @staticmethod
     def backward(ctx, g_table):
-        flat, raw, kind, first_reader, next_reader = ctx.saved_tensors
+        flat_in, raw, kind, first_reader, next_reader = ctx.saved_tensors
+        flat = flat_in.contiguous()
         g_table = g_table.contiguous()
         _require_cuda(g_table)
         g_flat = torch.empty_like(flat)
@@ -675,7 +712,7 @@ class FusedTableFunction(torch.autograd.Function):
                                                                _ptr(next_reader), _ptr(kind), raw.shape[0], flat.numel(),
                                                                _ptr(scratch), _ptr(g_flat), _stream())
         _check(rc, "drmb200_build_link_table_fused_backward")
-        return g_flat, None, None, None, None, None, None
+        return first_order_only((g_flat,), (flat_in, g_table)) + (None,) * 6
 
 
 class FkJacobianFunction(torch.autograd.Function):
@@ -683,15 +720,16 @@ class FkJacobianFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q, topo, ee_link, want_pos, want_quat, want_jac):
+        ctx.save_for_backward(table, q)  # as given, not the contiguous copies: first_order_only links to them
         table, q = table.contiguous(), q.contiguous()
         pos, quat, jlin, jang = fk_jacobian_raw(topo, ee_link, table, q, want_pos, want_quat, want_jac)
-        ctx.save_for_backward(table, q)
         ctx.topo, ctx.ee_link = topo, ee_link
         return pos, quat, jlin, jang           # skipped outputs are None
 
     @staticmethod
     def backward(ctx, g_pos, g_quat, g_jlin, g_jang):
-        table, q = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q = (t.contiguous() for t in saved)
         need_table, need_q = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         B, n = q.shape
         g = [None if t is None else t.contiguous() for t in (g_pos, g_quat, g_jlin, g_jang)]
@@ -704,7 +742,7 @@ class FkJacobianFunction(torch.autograd.Function):
                                                     _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(g[3]), _ptr(q_grad),
                                                     _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_fk_jacobian_backward")
-        return table_grad, q_grad, None, None, None, None, None
+        return first_order_only((table_grad, q_grad), saved + (g_pos, g_quat, g_jlin, g_jang)) + (None,) * 5
 
 
 class FkJacobianMultiFunction(torch.autograd.Function):
@@ -714,15 +752,16 @@ class FkJacobianMultiFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q, topo, ee_links, want_pos, want_quat, want_jac):
+        ctx.save_for_backward(table, q)  # as given, not the contiguous copies: first_order_only links to them
         table, q = table.contiguous(), q.contiguous()
         outs = fk_jacobian_multi_raw(topo, ee_links, table, q, want_pos, want_quat, want_jac)
-        ctx.save_for_backward(table, q)
         ctx.topo, ctx.ee_links = topo, tuple(ee_links)
         return outs
 
     @staticmethod
     def backward(ctx, g_pos, g_quat, g_jlin, g_jang):
-        table, q = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q = (t.contiguous() for t in saved)
         need_table, need_q = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         B, n = q.shape
         table_grad = torch.zeros_like(table) if need_table else None
@@ -741,7 +780,7 @@ class FkJacobianMultiFunction(torch.autograd.Function):
             _check(rc, "drmb200_fk_jacobian_backward")
             if need_q:
                 q_grad += q_grad_e
-        return table_grad, q_grad, None, None, None, None, None
+        return first_order_only((table_grad, q_grad), saved + (g_pos, g_quat, g_jlin, g_jang)) + (None,) * 5
 
 
 class AllLinksFkFunction(torch.autograd.Function):
@@ -750,9 +789,9 @@ class AllLinksFkFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q, topo):
+        ctx.save_for_backward(table, q)  # as given, not the contiguous copies: first_order_only links to them
         table, q = table.contiguous(), q.contiguous()
         poses, quats, _ = kinematic_state_raw(topo, table, q, None, want_poses=True, want_quats=True)
-        ctx.save_for_backward(table, q)
         ctx.topo = topo
         pos = poses[:, 9:12].transpose(1, 2).contiguous()       # [N, B, 3]
         quat = quats.transpose(1, 2).contiguous()               # [N, B, 4]
@@ -760,7 +799,8 @@ class AllLinksFkFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_pos, g_quat):
-        table, q = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q = (t.contiguous() for t in saved)
         need_table, need_q = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         B, n = q.shape
         N = ctx.topo.n_links
@@ -787,7 +827,7 @@ class AllLinksFkFunction(torch.autograd.Function):
             _check(rc, "drmb200_fk_jacobian_backward")
             if need_q:
                 q_grad += q_grad_l
-        return table_grad, q_grad, None
+        return first_order_only((table_grad, q_grad), saved + (g_pos, g_quat)) + (None,)
 
 
 class InverseDynamicsFunction(torch.autograd.Function):
@@ -795,15 +835,16 @@ class InverseDynamicsFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q, qd, qdd, topo, flags, folded=None):
+        ctx.save_for_backward(table, q, qd, qdd)  # as given, not the contiguous copies: first_order_only links to them
         table, q, qd, qdd = table.contiguous(), q.contiguous(), qd.contiguous(), qdd.contiguous()
         tau = inverse_dynamics_raw(topo, table, q, qd, qdd, flags, folded=folded)
-        ctx.save_for_backward(table, q, qd, qdd)
         ctx.topo, ctx.flags = topo, flags
         return tau
 
     @staticmethod
     def backward(ctx, g_tau):
-        table, q, qd, qdd = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q, qd, qdd = (t.contiguous() for t in saved)
         need = ctx.needs_input_grad
         B, n = q.shape
         g_tau = g_tau.contiguous()
@@ -821,7 +862,7 @@ class InverseDynamicsFunction(torch.autograd.Function):
                 ctypes.byref(ctx.topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(qdd), B, flags, _ptr(g_tau), _ptr(q_grad), _ptr(qd_grad), _ptr(qdd_grad),
                 _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_inverse_dynamics_backward")
-        return table_grad, q_grad, qd_grad, qdd_grad, None, None, None
+        return first_order_only((table_grad, q_grad, qd_grad, qdd_grad), saved + (g_tau,)) + (None,) * 3
 
 
 class ForwardDynamicsFunction(torch.autograd.Function):
@@ -829,15 +870,16 @@ class ForwardDynamicsFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q, qd, f, topo, flags, folded=None):
+        ctx.save_for_backward(table, q, qd, f)  # as given, not the contiguous copies: first_order_only links to them
         table, q, qd, f = table.contiguous(), q.contiguous(), qd.contiguous(), f.contiguous()
         qdd = forward_dynamics_raw(topo, table, q, qd, f, flags, folded=folded)
-        ctx.save_for_backward(table, q, qd, f)
         ctx.topo, ctx.flags = topo, flags
         return qdd
 
     @staticmethod
     def backward(ctx, g_qdd):
-        table, q, qd, f = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q, qd, f = (t.contiguous() for t in saved)
         need = ctx.needs_input_grad
         B, n = q.shape
         g_qdd = g_qdd.contiguous()
@@ -853,7 +895,7 @@ class ForwardDynamicsFunction(torch.autograd.Function):
                 ctypes.byref(ctx.topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B, ctx.flags, _ptr(g_qdd), _ptr(q_grad), _ptr(qd_grad),
                 _ptr(f_grad), _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_forward_dynamics_backward")
-        return table_grad, q_grad, qd_grad, f_grad, None, None, None
+        return first_order_only((table_grad, q_grad, qd_grad, f_grad), saved + (g_qdd,)) + (None,) * 3
 
 
 class ForwardDynamicsRolloutFunction(torch.autograd.Function):
@@ -862,15 +904,18 @@ class ForwardDynamicsRolloutFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q0, qd0, f, topo, flags, dt):
+        inputs = (table, q0, qd0, f)  # as given, not the contiguous copies: first_order_only links to them
         table, q0, qd0, f = table.contiguous(), q0.contiguous(), qd0.contiguous(), f.contiguous()
         q, qd, qdd = forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags)
-        ctx.save_for_backward(table, q0, qd0, f, q, qd)
+        ctx.save_for_backward(*inputs, q, qd)
         ctx.topo, ctx.flags, ctx.dt = topo, flags, dt
         return q, qd, qdd
 
     @staticmethod
     def backward(ctx, g_q, g_qd, g_qdd):
-        table, q0, qd0, f, q, qd = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q0, qd0, f = (t.contiguous() for t in saved[:4])
+        q, qd = saved[4:]
         need = ctx.needs_input_grad
         T, B, n = f.shape
         g = [None if t is None else t.contiguous() for t in (g_q, g_qd, g_qdd)]
@@ -888,7 +933,7 @@ class ForwardDynamicsRolloutFunction(torch.autograd.Function):
                 _ptr(q), _ptr(qd), _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(q0_grad), _ptr(qd0_grad), _ptr(f_grad),
                 _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_forward_dynamics_rollout_backward")
-        return table_grad, q0_grad, qd0_grad, f_grad, None, None, None
+        return first_order_only((table_grad, q0_grad, qd0_grad, f_grad), saved[:4] + (g_q, g_qd, g_qdd)) + (None,) * 3
 
 
 def mass_matrix_raw(topo, table, q, out=None, folded=None):
@@ -913,15 +958,16 @@ class MassMatrixFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, q, topo, folded=None):
+        ctx.save_for_backward(table, q)  # as given, not the contiguous copies: first_order_only links to them
         table, q = table.contiguous(), q.contiguous()
         H = mass_matrix_raw(topo, table, q, folded=folded)
-        ctx.save_for_backward(table, q)
         ctx.topo = topo
         return H
 
     @staticmethod
     def backward(ctx, g_H):
-        table, q = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        table, q = (t.contiguous() for t in saved)
         need_table, need_q = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         B, n = q.shape
         _require_cuda(g_H)
@@ -939,4 +985,5 @@ class MassMatrixFunction(torch.autograd.Function):
                 ctypes.byref(ctx.topo), _ptr(table), _ptr(qs), _ptr(zeros), _ptr(qdd.view(n * B, n)), n * B, 0, _ptr(g_tau),
                 _ptr(q_grad), None, None, _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_inverse_dynamics_backward")
-        return table_grad, (q_grad.view(n, B, n).sum(0) if need_q else None), None, None
+        q_grad = q_grad.view(n, B, n).sum(0) if need_q else None
+        return first_order_only((table_grad, q_grad), saved + (g_H,)) + (None,) * 2
