@@ -102,6 +102,14 @@ int64_t forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology
 int forward_dynamics_rollout_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*,
                                              int64_t, int32_t, float, uint32_t, const float*, const float*, const float*,
                                              const float*, const float*, float*, float*, float*, float*, void*, cudaStream_t);
+int pd_rollout_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, const float*, const float*,
+                      const float*, const float*, int32_t, const float*, int64_t, int32_t, float, uint32_t, float*, float*, float*,
+                      float*, cudaStream_t);
+int64_t pd_rollout_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
+int pd_rollout_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, const float*,
+                               const float*, const float*, const float*, int32_t, const float*, int64_t, int32_t, float, uint32_t,
+                               const float*, const float*, const float*, const float*, const float*, const float*, const float*,
+                               float*, float*, float*, float*, float*, float*, float*, float*, void*, cudaStream_t);
 int inverse_dynamics_derivatives_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
                                         uint32_t, float*, float*, cudaStream_t, bool);
 int forward_dynamics_derivatives_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
@@ -395,6 +403,31 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
     return drm::forward_dynamics_rollout_backward_device(topo, table, q0, qd0, f, batch, n_steps, dt, flags, q, qd, g_q, g_qd,
                                                          g_qdd, q0_grad, qd0_grad, f_grad, table_grad, workspace,
                                                          static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_pd_rollout(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
+                       const float* q_ref, const float* qd_ref, const float* f, const float* kp, const float* kd,
+                       int32_t gains_per_row, const float* effort_limit, int64_t batch, int32_t n_steps, float dt,
+                       uint32_t flags, float* q, float* qd, float* qdd, float* tau, void* cuda_stream) {
+    return drm::pd_rollout_device(topo, table, q0, qd0, q_ref, qd_ref, f, kp, kd, gains_per_row, effort_limit, batch, n_steps,
+                                  dt, flags, q, qd, qdd, tau, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int64_t drmb200_pd_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
+    return drm::pd_rollout_backward_workspace_bytes(topo, batch);
+}
+
+int drmb200_pd_rollout_backward(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
+                                const float* q_ref, const float* qd_ref, const float* f, const float* kp, const float* kd,
+                                int32_t gains_per_row, const float* effort_limit, int64_t batch, int32_t n_steps, float dt,
+                                uint32_t flags, const float* q, const float* qd, const float* tau, const float* g_q,
+                                const float* g_qd, const float* g_qdd, const float* g_tau, float* q0_grad, float* qd0_grad,
+                                float* q_ref_grad, float* qd_ref_grad, float* f_grad, float* kp_grad, float* kd_grad,
+                                float* table_grad, void* workspace, void* cuda_stream) {
+    return drm::pd_rollout_backward_device(topo, table, q0, qd0, q_ref, qd_ref, f, kp, kd, gains_per_row, effort_limit, batch,
+                                           n_steps, dt, flags, q, qd, tau, g_q, g_qd, g_qdd, g_tau, q0_grad, qd0_grad,
+                                           q_ref_grad, qd_ref_grad, f_grad, kp_grad, kd_grad, table_grad, workspace,
+                                           static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_inverse_dynamics_derivatives(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

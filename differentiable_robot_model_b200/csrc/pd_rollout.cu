@@ -1,0 +1,430 @@
+// pd_rollout.cu -- batched PD-controlled rollouts (sm_90a): the forward-dynamics rollout of rollout.cu with a diagonal
+// joint-space PD law closing the loop inside the same launch, and its reverse-time adjoint.
+//
+// Step t, fp32, every operation rounded separately (the definition is stated in include/drm_b200.h):
+//   e_t = q_ref[t] - q_t;  ed_t = qd_ref[t] - qd_t;  u_t = (f[t] + kp e_t) + kd ed_t;  tau_t = clamp(u_t, -lim, lim)
+//   qdd_t = FD(q_t, qd_t, tau_t), then rollout.cu's integrate.  (qd_ref / f absent: 0 - qd_t / 0 + kp e_t; lim absent: no
+//   clamp.)
+// pd_rollout_kernel<T> is a sibling of rollout_kernel<T>: the same per-thread body (aba_body.cuh), staging helpers and
+// 64 / 32 tile rule, in a translation unit of its own so that the open-loop kernels compile exactly as before.  Per step the q_ref /
+// qd_ref / f tiles arrive by TMA in ONE mbarrier transaction into a double buffer, exactly as f does there; per-row gains
+// are staged once per CTA, shared gains and limits once as [n] rows.  Each thread forms its tau_t row from the live s_q /
+// s_qd into a SEPARATE double-buffered tau tile, which aba_body reads as its f and which leaves by bulk store beside q / qd /
+// qdd.  Ordering: the tau tile of step t is rewritten at step t + 2, after thread 0's bulk_wait_read at step t + 1 (the one
+// that already guards s_q / s_qd / s_qdd) and the barrier after it, so the store of step t has read it; the threads'
+// generic writes to it are ordered before its bulk store by the fence_proxy_async that precedes every store.  The input
+// buffer is only read (by the tau formation), so its prefetch needs no more ordering than f's.
+// Algorithmic HBM bytes per configuration-step: q_ref 4n (+ qd_ref 4n, + f 4n) in, q / qd / qdd / tau 16n out: up to 28n.
+//
+// Adjoint (drmb200_pd_rollout_backward): the open-loop adjoint with the feedback folded into the element-wise step.  With
+// gu_t = mask_t (gf_t + g_tau[t]), mask_t = (-lim <= u_t <= lim) (1 without a limit; u_t recomputed bit-exactly), the
+// post-update of step t becomes
+//   a_q = (a_q + gq) - kp gu_t;  a_qd = (a_qd' + gqd) - kd gu_t;  f_grad[t] = gu_t;  q_ref_grad[t] = kp gu_t;
+//   qd_ref_grad[t] = kd gu_t;  kp_grad += gu_t e_t;  kd_grad += gu_t ed_t      (kp_grad / kd_grad per row, [B, n])
+// still 2T + 2 launches, no atomics.
+#include "aba_body.cuh"
+#include "launch.cuh"
+
+namespace drm {
+
+int forward_dynamics_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
+                                     uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t, bool, bool);
+int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
+
+// u = (f + kp e) + kd ed with e = q_ref - q, ed = qd_ref - qd: the rounding of the torch expression
+// `f + kp * (q_ref - q) + kd * (qd_ref - qd)`; pass 0.f for an absent f / qd_ref (a zero tensor, -0 included)
+__device__ __forceinline__ float pd_command(float q_ref, float q, float qd_ref, float qd, float f, float kp, float kd,
+                                            float& e, float& ed) {
+    e = __fsub_rn(q_ref, q);
+    ed = __fsub_rn(qd_ref, qd);
+    return __fadd_rn(__fadd_rn(f, __fmul_rn(kp, e)), __fmul_rn(kd, ed));
+}
+
+// torch.clamp(u, -lim, lim): NaN propagates
+__device__ __forceinline__ float pd_clamp(float u, float lim) {
+    return isnan(u) ? u : fminf(fmaxf(u, -lim), lim);
+}
+
+struct PDRolloutArgs {
+    const float* __restrict__ table;
+    const float* __restrict__ q0;
+    const float* __restrict__ qd0;
+    const float* __restrict__ q_ref;
+    const float* __restrict__ qd_ref;   // may be null
+    const float* __restrict__ f;        // may be null
+    const float* __restrict__ kp;       // [n] or [B, n]
+    const float* __restrict__ kd;
+    const float* __restrict__ lim;      // [n], may be null
+    float* __restrict__ q;
+    float* __restrict__ qd;
+    float* __restrict__ qdd;            // may be null
+    float* __restrict__ tau;
+    int64_t batch;
+    int32_t n_steps;
+    float dt;
+    uint32_t flags;
+    int32_t per_row;                    // kp / kd are [B, n]
+    int32_t aligned;                    // as RolloutArgs, over every tile pointer (and kp / kd when per row)
+};
+
+struct PDRolloutSmem {
+    int q, qd, in, tau, qdd, kp, kd, lim, table, link, slots, total_floats;
+    // n_in input tiles per step (q_ref, then qd_ref and f when given); every region starts 16-byte aligned
+    __host__ __device__ PDRolloutSmem(int T, int n, int n_links, int n_slots, int n_in, bool per_row) {
+        const int gain = ((per_row ? T : 1) * n + 3) & ~3;
+        int o = 0;
+        q = o;   o += T * n;
+        qd = o;  o += T * n;
+        in = o;  o += 2 * n_in * T * n;  // double buffer
+        tau = o; o += 2 * T * n;         // double buffer
+        qdd = o; o += 2 * T * n;         // double buffer
+        kp = o;  o += gain;
+        kd = o;  o += gain;
+        lim = o; o += (n + 3) & ~3;
+        table = o; o += n_links * DRMB200_TABLE_STRIDE;
+        link = o;  o += n_links * ABA_LINK * T;
+        slots = o; o += n_slots * ABA_SLOT * T;
+        total_floats = o;
+    }
+};
+
+template <int T>
+__global__ void __launch_bounds__(T)
+pd_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const PDRolloutArgs args) {
+    extern __shared__ __align__(128) float smem[];
+    __shared__ __align__(8) uint64_t mbar[2];
+
+    const int n = prog.n_dofs;
+    const int N = prog.n_links;
+    const bool has_qdr = args.qd_ref != nullptr, has_f = args.f != nullptr, has_lim = args.lim != nullptr;
+    const int n_in = 1 + (int)has_qdr + (int)has_f;
+    const PDRolloutSmem L(T, n, N, prog.n_slots, n_in, args.per_row != 0);
+    float* s_q = smem + L.q;
+    float* s_qd = smem + L.qd;
+    float* s_in = smem + L.in;
+    float* s_tau = smem + L.tau;
+    float* s_qdd = smem + L.qdd;
+    float* s_kp = smem + L.kp;
+    float* s_kd = smem + L.kd;
+    float* s_lim = smem + L.lim;
+    float* s_tab = smem + L.table;
+    float* s_link = smem + L.link;
+    float* s_slot = smem + L.slots;
+
+    const int tid = threadIdx.x;
+    const int64_t tile_off = (int64_t)blockIdx.x * T * n;
+    const int valid = (int)min((int64_t)T, args.batch - (int64_t)blockIdx.x * T);
+    const int tile_floats = valid * n;
+    const int64_t step = args.batch * n;
+    const bool vec_ok = args.aligned;
+    const bool bulk = args.aligned && ((tile_floats & 3) == 0);
+    const uint32_t bytes = (uint32_t)tile_floats * 4u;
+    const int o_f = (has_qdr ? 2 : 1) * T * n;          // slots of one input buffer: q_ref | qd_ref | f
+
+    // the input tiles of step t into buffer `dst` (thread 0, TMA) or cooperatively
+    auto issue_inputs = [&](int t, float* dst, uint64_t* bar) {
+        const int64_t off = (int64_t)t * step + tile_off;
+        bulk_g2s(dst, args.q_ref + off, bytes, bar);
+        if (has_qdr) bulk_g2s(dst + T * n, args.qd_ref + off, bytes, bar);
+        if (has_f) bulk_g2s(dst + o_f, args.f + off, bytes, bar);
+    };
+    if (bulk) {
+        if (tid == 0) {
+            mbar_init(&mbar[0], 1);
+            mbar_init(&mbar[1], 1);
+            fence_mbar_init();
+            mbar_arrive_expect_tx(&mbar[0], (uint32_t)(2 + n_in) * bytes);
+            bulk_g2s(s_q, args.q0 + tile_off, bytes, &mbar[0]);
+            bulk_g2s(s_qd, args.qd0 + tile_off, bytes, &mbar[0]);
+            issue_inputs(0, s_in, &mbar[0]);
+        }
+    } else {
+        coop_copy(s_q, args.q0 + tile_off, tile_floats, vec_ok);
+        coop_copy(s_qd, args.qd0 + tile_off, tile_floats, vec_ok);
+    }
+    if (args.per_row) {
+        coop_copy(s_kp, args.kp + tile_off, tile_floats, vec_ok);
+        coop_copy(s_kd, args.kd + tile_off, tile_floats, vec_ok);
+    } else {
+        coop_copy(s_kp, args.kp, n, false);
+        coop_copy(s_kd, args.kd, n, false);
+    }
+    if (has_lim) coop_copy(s_lim, args.lim, n, false);
+    if (fold.n_red > 0) stage_folded_table(s_tab, s_link, args.table, fold, prog, T);
+    else stage_canonical_table(s_tab, args.table, prog, T);
+    __syncthreads();
+
+    const float dt = args.dt;
+    const int gain_row = args.per_row ? tid * n : 0;
+    for (int t = 0; t < args.n_steps; ++t) {
+        const int b = t & 1;
+        float* s_it = s_in + b * n_in * T * n;
+        float* s_taut = s_tau + b * T * n;
+        float* s_qddt = s_qdd + b * T * n;
+        if (bulk) {
+            // buffer b ^ 1 was last read by the tau formation of step t - 1, which every thread finished (and fenced
+            // against the async proxy) before the barrier that ended step t - 1
+            if (tid == 0 && t + 1 < args.n_steps) {
+                mbar_arrive_expect_tx(&mbar[b ^ 1], (uint32_t)n_in * bytes);
+                issue_inputs(t + 1, s_in + (b ^ 1) * n_in * T * n, &mbar[b ^ 1]);
+            }
+            mbar_wait(&mbar[b], (uint32_t)(t >> 1) & 1u);
+        } else {
+            const int64_t off = (int64_t)t * step + tile_off;
+            coop_copy(s_it, args.q_ref + off, tile_floats, vec_ok);
+            if (has_qdr) coop_copy(s_it + T * n, args.qd_ref + off, tile_floats, vec_ok);
+            if (has_f) coop_copy(s_it + o_f, args.f + off, tile_floats, vec_ok);
+            __syncthreads();
+        }
+
+        if (tid < valid) {
+            const float* qr = s_q + tid * n;
+            const float* qdr = s_qd + tid * n;
+            const float* ref = s_it + tid * n;
+            float* taur = s_taut + tid * n;
+            for (int k = 0; k < n; ++k) {
+                float e, ed;
+                const float u = pd_command(ref[k], qr[k], has_qdr ? ref[T * n + k] : 0.f, qdr[k], has_f ? ref[o_f + k] : 0.f,
+                                           s_kp[gain_row + k], s_kd[gain_row + k], e, ed);
+                taur[k] = has_lim ? pd_clamp(u, s_lim[k]) : u;
+            }
+            aba_body<T>(prog, s_tab, s_q + tid * n, s_qd + tid * n, taur, s_qddt + tid * n, s_link + tid, s_slot + tid,
+                        args.flags);
+        }
+
+        if (bulk) {
+            if (tid == 0) bulk_wait_read<0>();           // the stores of step t - 1 have read s_q / s_qd / its tau, qdd
+            __syncthreads();
+        }
+        if (tid < valid) {
+            float* qr = s_q + tid * n;
+            float* qdr = s_qd + tid * n;
+            const float* ar = s_qddt + tid * n;
+            for (int k = 0; k < n; ++k) {
+                const float v = __fadd_rn(qdr[k], __fmul_rn(dt, ar[k]));
+                qdr[k] = v;
+                qr[k] = __fadd_rn(qr[k], __fmul_rn(dt, v));
+            }
+        }
+        const int64_t out_off = (int64_t)t * step + tile_off;
+        if (bulk) {
+            fence_proxy_async();
+            __syncthreads();
+            if (tid == 0) {
+                bulk_s2g(args.q + out_off, s_q, bytes);
+                bulk_s2g(args.qd + out_off, s_qd, bytes);
+                bulk_s2g(args.tau + out_off, s_taut, bytes);
+                if (args.qdd != nullptr) bulk_s2g(args.qdd + out_off, s_qddt, bytes);
+                bulk_commit();
+            }
+        } else {
+            __syncthreads();
+            coop_copy(args.q + out_off, s_q, tile_floats, vec_ok);
+            coop_copy(args.qd + out_off, s_qd, tile_floats, vec_ok);
+            coop_copy(args.tau + out_off, s_taut, tile_floats, vec_ok);
+            if (args.qdd != nullptr) coop_copy(args.qdd + out_off, s_qddt, tile_floats, vec_ok);
+            // the next step's tau formation reads s_q / s_qd only after the barrier that follows its input copies
+        }
+    }
+    if (bulk && tid == 0) bulk_wait_read<0>();
+}
+
+// the element-wise update between two ABA adjoint launches: the post-update of step s = t + 1 (feedback included) fused
+// with the pre-update of step t, as rollout_adjoint_step_kernel
+struct PDAdjStepArgs {
+    float* a_q;                 // running adjoints of q_t / qd_t  [B, n]
+    float* a_qd;
+    float* g_step;              // g_qdd_t handed to the ABA adjoint
+    const float* gq;            // ABA adjoint of step s (post-update; unused when first)
+    const float* gqd;
+    const float* gf;
+    // step s of the post-update: its state, inputs, upstream g_tau (NULL = zero) and outputs (NULL = not wanted)
+    const float* qs;
+    const float* qds;
+    const float* q_ref;
+    const float* qd_ref;
+    const float* f;
+    const float* g_tau;
+    float* f_grad;
+    float* q_ref_grad;
+    float* qd_ref_grad;
+    float* kp_grad;             // [B, n] running sums over the steps (NULL = not wanted)
+    float* kd_grad;
+    const float* kp;
+    const float* kd;
+    const float* lim;
+    int32_t n;
+    int32_t per_row;
+    int32_t last_post;          // s = T - 1: kp_grad / kd_grad are written rather than accumulated
+    // step t of the pre-update
+    const float* g_q;
+    const float* g_qd;
+    const float* g_qdd;
+    float* out_q;               // final: q0_grad / qd0_grad (NULL = not wanted)
+    float* out_qd;
+    int64_t count;
+    float dt;
+    int32_t first;              // t = T - 1: the running adjoints start at zero
+    int32_t final;              // after step 0: post-update only, written to out_q / out_qd
+};
+
+__global__ void __launch_bounds__(256) pd_rollout_adjoint_step_kernel(const PDAdjStepArgs a) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.count; i += (int64_t)gridDim.x * blockDim.x) {
+        float aq = 0.f, aqd = 0.f;
+        if (!a.first) {                                        // post-update of step s
+            const int k = (int)(i % a.n);
+            const int64_t gi = a.per_row ? i : k;
+            const float kp = a.kp[gi], kd = a.kd[gi];
+            float e, ed;
+            const float u = pd_command(a.q_ref[i], a.qs[i], a.qd_ref ? a.qd_ref[i] : 0.f, a.qds[i], a.f ? a.f[i] : 0.f, kp, kd,
+                                       e, ed);
+            float gu = a.gf[i];
+            if (a.g_tau != nullptr) gu = __fadd_rn(gu, a.g_tau[i]);
+            if (a.lim != nullptr && !(u >= -a.lim[k] && u <= a.lim[k])) gu = 0.f;   // torch.clamp's rule: equality passes
+            aq = __fsub_rn(__fadd_rn(a.a_q[i], a.gq[i]), __fmul_rn(kp, gu));
+            aqd = __fsub_rn(__fadd_rn(a.a_qd[i], a.gqd[i]), __fmul_rn(kd, gu));
+            if (a.f_grad != nullptr) a.f_grad[i] = gu;
+            if (a.q_ref_grad != nullptr) a.q_ref_grad[i] = __fmul_rn(kp, gu);
+            if (a.qd_ref_grad != nullptr) a.qd_ref_grad[i] = __fmul_rn(kd, gu);
+            if (a.kp_grad != nullptr) a.kp_grad[i] = a.last_post ? __fmul_rn(gu, e) : __fadd_rn(a.kp_grad[i], __fmul_rn(gu, e));
+            if (a.kd_grad != nullptr) a.kd_grad[i] = a.last_post ? __fmul_rn(gu, ed) : __fadd_rn(a.kd_grad[i], __fmul_rn(gu, ed));
+        }
+        if (a.final) {
+            if (a.out_q != nullptr) a.out_q[i] = aq;
+            if (a.out_qd != nullptr) a.out_qd[i] = aqd;
+            continue;
+        }
+        if (a.g_q != nullptr) aq = __fadd_rn(aq, a.g_q[i]);    // pre-update of step t
+        if (a.g_qd != nullptr) aqd = __fadd_rn(aqd, a.g_qd[i]);
+        aqd = __fadd_rn(aqd, __fmul_rn(a.dt, aq));             // a_qd' = a_qd + dt a_q
+        float g = __fmul_rn(a.dt, aqd);
+        if (a.g_qdd != nullptr) g = __fadd_rn(g, a.g_qdd[i]);
+        a.a_q[i] = aq;
+        a.a_qd[i] = aqd;
+        a.g_step[i] = g;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------
+static int64_t round256(int64_t bytes) { return (bytes + 255) & ~(int64_t)255; }
+
+int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0, const float* q_ref,
+                      const float* qd_ref, const float* f, const float* kp, const float* kd, int32_t gains_per_row,
+                      const float* effort_limit, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q, float* qd,
+                      float* qdd, float* tau, cudaStream_t stream) {
+    FoldChoice fc;
+    const int rc = select_fold(topo, false, &fc);                   // "rnea_fold", as drmb200_forward_dynamics
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
+    if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
+    if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
+    if (batch == 0 || n_steps == 0 || prog.n_dofs == 0) return DRMB200_OK;
+    if (table == nullptr || q0 == nullptr || qd0 == nullptr || q_ref == nullptr || kp == nullptr || kd == nullptr ||
+        q == nullptr || qd == nullptr || tau == nullptr) {
+        set_error("null pointer argument");
+        return DRMB200_EINVAL;
+    }
+
+    PDRolloutArgs args;
+    args.table = table; args.q0 = q0; args.qd0 = qd0; args.q_ref = q_ref; args.qd_ref = qd_ref; args.f = f;
+    args.kp = kp; args.kd = kd; args.lim = effort_limit; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau;
+    args.batch = batch; args.n_steps = n_steps; args.dt = dt; args.flags = flags; args.per_row = gains_per_row;
+    args.aligned = aligned16(q0, qd0, q_ref, qd_ref, f, q, qd, qdd, tau) && (!gains_per_row || aligned16(kp, kd)) &&
+                   ((batch * prog.n_dofs) & 3) == 0;
+
+    const int n_in = 1 + (qd_ref != nullptr) + (f != nullptr);
+    // the open-loop rollout's tile rule, on this kernel's shared memory
+    const TileChoice c = tile_64_or_32([&](int T) {
+        return (size_t)PDRolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots, n_in, gains_per_row != 0).total_floats * sizeof(float);
+    }, 0, (batch + 63) / 64 >= device_sm_count());
+    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
+    const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    return c.tile == 64 ? launch_kernel<pd_rollout_kernel<64>>(tiles, 64, c.bytes, stream, false, "pd rollout", prog, fc.fold, args)
+                        : launch_kernel<pd_rollout_kernel<32>>(tiles, 32, c.bytes, stream, false, "pd rollout", prog, fc.fold, args);
+}
+
+// [ABA adjoint workspace | a_q | a_qd | g_qdd_t | gq | gqd | gf], each [B, n] fp32
+int64_t pd_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
+    if (topo == nullptr || topo->n_links < 1 || topo->n_links > DRMB200_MAX_LINKS || batch < 0) return 0;
+    return round256(forward_dynamics_backward_workspace_bytes(topo, batch)) + 6 * round256(batch * topo->n_dofs * (int64_t)sizeof(float));
+}
+
+int pd_rollout_backward_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
+                               const float* q_ref, const float* qd_ref, const float* f, const float* kp, const float* kd,
+                               int32_t gains_per_row, const float* effort_limit, int64_t batch, int32_t n_steps, float dt,
+                               uint32_t flags, const float* q, const float* qd, const float* tau, const float* g_q,
+                               const float* g_qd, const float* g_qdd, const float* g_tau, float* q0_grad, float* qd0_grad,
+                               float* q_ref_grad, float* qd_ref_grad, float* f_grad, float* kp_grad, float* kd_grad,
+                               float* table_grad, void* workspace, cudaStream_t stream) {
+    if (topo == nullptr) { set_error("null topology"); return DRMB200_EINVAL; }
+    if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
+    if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
+    if (batch == 0 || n_steps == 0 || topo->n_dofs == 0) return DRMB200_OK;
+    const bool want_elementwise = q0_grad || qd0_grad || q_ref_grad || qd_ref_grad || f_grad || kp_grad || kd_grad;
+    if (!want_elementwise && table_grad == nullptr) return DRMB200_OK;
+    if (table == nullptr || q0 == nullptr || qd0 == nullptr || q_ref == nullptr || kp == nullptr || kd == nullptr ||
+        tau == nullptr || (n_steps > 1 && (q == nullptr || qd == nullptr))) {
+        set_error("null pointer argument");
+        return DRMB200_EINVAL;
+    }
+    if (workspace == nullptr) { set_error("pd rollout backward needs its workspace (drmb200_pd_rollout_backward_workspace_bytes)"); return DRMB200_EINVAL; }
+
+    const int64_t count = batch * topo->n_dofs;
+    const int64_t slice = round256(count * (int64_t)sizeof(float));
+    char* ws = static_cast<char*>(workspace);
+    void* fd_ws = ws;
+    ws += round256(forward_dynamics_backward_workspace_bytes(topo, batch));
+    float* a_q = reinterpret_cast<float*>(ws);
+    float* a_qd = reinterpret_cast<float*>(ws + slice);
+    float* g_step = reinterpret_cast<float*>(ws + 2 * slice);
+    float* gq = reinterpret_cast<float*>(ws + 3 * slice);
+    float* gqd = reinterpret_cast<float*>(ws + 4 * slice);
+    float* gf = reinterpret_cast<float*>(ws + 5 * slice);
+
+    int64_t blocks = (count + 255) / 256;
+    if (blocks > (int64_t)device_sm_count() * 8) blocks = (int64_t)device_sm_count() * 8;
+    auto step_kernel = [&](const PDAdjStepArgs& a) {
+        return launch_kernel<pd_rollout_adjoint_step_kernel>(blocks, 256, 0, stream, false, "pd rollout adjoint step", a);
+    };
+    auto at = [&](auto* p, int s) { return p ? p + (int64_t)s * count : nullptr; };
+
+    PDAdjStepArgs a = {};
+    a.a_q = a_q; a.a_qd = a_qd; a.g_step = g_step; a.gq = gq; a.gqd = gqd; a.gf = gf;
+    a.kp_grad = kp_grad; a.kd_grad = kd_grad; a.kp = kp; a.kd = kd; a.lim = effort_limit;
+    a.n = topo->n_dofs; a.per_row = gains_per_row; a.count = count; a.dt = dt;
+    // the post-update of step s reads its state (q0 / qd0, then the forward's outputs) and inputs, writes its gradients
+    auto post = [&](int s) {
+        a.qs = s == 0 ? q0 : q + (int64_t)(s - 1) * count;
+        a.qds = s == 0 ? qd0 : qd + (int64_t)(s - 1) * count;
+        a.q_ref = at(q_ref, s); a.qd_ref = at(qd_ref, s); a.f = at(f, s); a.g_tau = at(g_tau, s);
+        a.f_grad = at(f_grad, s); a.q_ref_grad = at(q_ref_grad, s); a.qd_ref_grad = at(qd_ref_grad, s);
+        a.last_post = s == n_steps - 1;
+    };
+    for (int t = n_steps - 1; t >= 0; --t) {
+        a.first = (t == n_steps - 1) ? 1 : 0;
+        a.final = 0;
+        if (!a.first) post(t + 1);
+        a.g_q = at(g_q, t);
+        a.g_qd = at(g_qd, t);
+        a.g_qdd = at(g_qdd, t);
+        int rc = step_kernel(a);
+        if (rc != DRMB200_OK) return rc;
+        const float* qt = t == 0 ? q0 : q + (int64_t)(t - 1) * count;
+        const float* qdt = t == 0 ? qd0 : qd + (int64_t)(t - 1) * count;
+        rc = forward_dynamics_backward_device(topo, table, qt, qdt, tau + (int64_t)t * count, batch, flags, g_step, gq, gqd, gf,
+                                              table_grad, fd_ws, stream, /*accumulate_partials=*/t != n_steps - 1,
+                                              /*reduce=*/t == 0);
+        if (rc != DRMB200_OK) return rc;
+    }
+    if (!want_elementwise) return DRMB200_OK;
+    a.first = 0;
+    a.final = 1;
+    post(0);
+    a.out_q = q0_grad;
+    a.out_qd = qd0_grad;
+    return step_kernel(a);
+}
+
+}  // namespace drm

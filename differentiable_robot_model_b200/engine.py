@@ -78,6 +78,17 @@ _SIGNATURES = {
                                                                  ctypes.c_uint32, _c_float_p, _c_float_p, _c_float_p,
                                                                  _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                                  _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_pd_rollout": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                          _c_float_p, _c_float_p, _c_float_p, ctypes.c_int32, _c_float_p, ctypes.c_int64,
+                                          ctypes.c_int32, ctypes.c_float, ctypes.c_uint32, _c_float_p, _c_float_p, _c_float_p,
+                                          _c_float_p, ctypes.c_void_p]),
+    "drmb200_pd_rollout_backward_workspace_bytes": (ctypes.c_int64, [ctypes.POINTER(Topology), ctypes.c_int64]),
+    "drmb200_pd_rollout_backward": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                   _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int32, _c_float_p,
+                                                   ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_uint32, _c_float_p,
+                                                   _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                   _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                   _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
     "drmb200_inverse_dynamics_derivatives": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
                                                             _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p, _c_float_p,
                                                             ctypes.c_void_p]),
@@ -411,6 +422,27 @@ def forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags, want_qdd=Tr
                                                     ctypes.c_float(dt), flags, _ptr(q), _ptr(qd), _ptr(qdd), _stream())
     _check(rc, "drmb200_forward_dynamics_rollout")
     return q, qd, qdd
+
+
+def pd_rollout_raw(topo, table, q0, qd0, q_ref, kp, kd, dt, flags, qd_ref=None, f=None, effort_limit=None, want_qdd=True):
+    """(q, qd, qdd, tau) [T, B, n] of T semi-implicit Euler steps over the articulated-body algorithm driven by the PD law
+    tau = clamp(f + kp (q_ref - q) + kd (qd_ref - qd), -effort_limit, effort_limit), one launch (drmb200_pd_rollout).
+    kp / kd both [n] (shared) or both [B, n] (per row); qd_ref, f, effort_limit may be None; qdd is None unless want_qdd."""
+    _require_cuda(table, q0, qd0, q_ref, kp, kd, qd_ref, f, effort_limit)
+    if kp.shape != kd.shape:      # one gains_per_row flag describes both buffers
+        raise RuntimeError(f"kp and kd must have the same shape (got {tuple(kp.shape)} and {tuple(kd.shape)})")
+    q0, qd0, q_ref, kp, kd = (t.contiguous() for t in (q0, qd0, q_ref, kp, kd))
+    qd_ref, f, effort_limit = (None if t is None else t.contiguous() for t in (qd_ref, f, effort_limit))
+    T, B, n = q_ref.shape
+    dev = q0.device
+    q, qd, tau = (torch.empty((T, B, n), device=dev, dtype=torch.float32) for _ in range(3))
+    qdd = torch.empty((T, B, n), device=dev, dtype=torch.float32) if want_qdd else None
+    with _on(dev):
+        rc = lib().drmb200_pd_rollout(ctypes.byref(topo), _ptr(table), _ptr(q0), _ptr(qd0), _ptr(q_ref), _ptr(qd_ref), _ptr(f),
+                                      _ptr(kp), _ptr(kd), 1 if kp.ndim == 2 else 0, _ptr(effort_limit), B, T, ctypes.c_float(dt),
+                                      flags, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(tau), _stream())
+    _check(rc, "drmb200_pd_rollout")
+    return q, qd, qdd, tau
 
 
 IK_DAMPING_INIT = 1e-2       # suggested initial Levenberg-Marquardt damping (include/drm_b200.h)
@@ -934,6 +966,57 @@ class ForwardDynamicsRolloutFunction(torch.autograd.Function):
                 _ptr(table_grad), _ptr(ws), _stream())
         _check(rc, "drmb200_forward_dynamics_rollout_backward")
         return first_order_only((table_grad, q0_grad, qd0_grad, f_grad), saved[:4] + (g_q, g_qd, g_qdd)) + (None,) * 3
+
+
+class PDRolloutFunction(torch.autograd.Function):
+    """(table, q0, qd0, q_ref, qd_ref, f, kp, kd) -> (q, qd, qdd, tau) of a PD-controlled rollout; one launch forward, the ABA
+    adjoint stepped in reverse time with the feedback folded into the element-wise step backward
+    (drmb200_pd_rollout_backward).  qd_ref / f may be None; not differentiable in dt or effort_limit.  The kernel returns
+    the gains' gradients per row; a shared gain's is their sum over rows, a fixed-order torch reduction."""
+
+    @staticmethod
+    def forward(ctx, table, q0, qd0, q_ref, qd_ref, f, kp, kd, topo, flags, dt, effort_limit):
+        inputs = (table, q0, qd0, q_ref, qd_ref, f, kp, kd)  # as given: first_order_only links to them
+        q, qd, qdd, tau = pd_rollout_raw(topo, table.contiguous(), q0, qd0, q_ref, kp, kd, dt, flags, qd_ref, f, effort_limit)
+        ctx.has = tuple(t is not None for t in inputs)
+        ctx.save_for_backward(*[t for t in inputs if t is not None], effort_limit, q, qd, tau)
+        ctx.topo, ctx.flags, ctx.dt = topo, flags, dt
+        return q, qd, qdd, tau
+
+    @staticmethod
+    def backward(ctx, g_q, g_qd, g_qdd, g_tau):
+        saved = list(ctx.saved_tensors)
+        given = [saved.pop(0) if has else None for has in ctx.has]
+        effort_limit, q, qd, tau = saved
+        table, q0, qd0, q_ref, qd_ref, f, kp, kd = (None if t is None else t.contiguous() for t in given)
+        need = ctx.needs_input_grad
+        T, B, n = q_ref.shape
+        g = [None if t is None else t.contiguous() for t in (g_q, g_qd, g_qdd, g_tau)]
+        _require_cuda(*g)
+        per_row = kp.ndim == 2
+        table_grad = torch.zeros_like(table) if need[0] else None
+        alloc = torch.zeros_like if T == 0 else torch.empty_like       # zero steps: nothing reaches the inputs
+        q0_grad = alloc(q0) if need[1] else None
+        qd0_grad = alloc(q0) if need[2] else None
+        q_ref_grad = torch.empty_like(q_ref) if need[3] else None
+        qd_ref_grad = torch.empty_like(q_ref) if need[4] else None
+        f_grad = torch.empty_like(q_ref) if need[5] else None
+        kp_rows = alloc(q0) if need[6] else None                       # [B, n] per row, whichever the gains' shape
+        kd_rows = alloc(q0) if need[7] else None
+        nbytes = int(lib().drmb200_pd_rollout_backward_workspace_bytes(ctypes.byref(ctx.topo), B))
+        ws = torch.empty((max(nbytes, 4) + 3) // 4, device=q0.device, dtype=torch.float32)
+        with _on(q0.device):
+            rc = lib().drmb200_pd_rollout_backward(
+                ctypes.byref(ctx.topo), _ptr(table), _ptr(q0), _ptr(qd0), _ptr(q_ref), _ptr(qd_ref), _ptr(f), _ptr(kp), _ptr(kd),
+                1 if per_row else 0, _ptr(effort_limit), B, T, ctypes.c_float(ctx.dt), ctx.flags, _ptr(q), _ptr(qd), _ptr(tau),
+                _ptr(g[0]), _ptr(g[1]), _ptr(g[2]), _ptr(g[3]), _ptr(q0_grad), _ptr(qd0_grad), _ptr(q_ref_grad),
+                _ptr(qd_ref_grad), _ptr(f_grad), _ptr(kp_rows), _ptr(kd_rows), _ptr(table_grad), _ptr(ws), _stream())
+        _check(rc, "drmb200_pd_rollout_backward")
+        kp_grad = kp_rows if per_row or kp_rows is None else kp_rows.sum(0)
+        kd_grad = kd_rows if per_row or kd_rows is None else kd_rows.sum(0)
+        grads = (table_grad, q0_grad, qd0_grad, q_ref_grad, qd_ref_grad, f_grad, kp_grad, kd_grad)
+        deps = tuple(t for t in given if t is not None) + (g_q, g_qd, g_qdd, g_tau)
+        return first_order_only(grads, deps) + (None,) * 4
 
 
 def mass_matrix_raw(topo, table, q, out=None, folded=None):

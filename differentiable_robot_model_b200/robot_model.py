@@ -24,6 +24,7 @@ Deliberate deviations from the reference (see DESIGN.md):
 """
 import contextlib
 import os
+import weakref
 from dataclasses import dataclass
 from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
@@ -133,6 +134,16 @@ class EnergyAndMomentum(NamedTuple):
     com: torch.Tensor
     com_velocity: Optional[torch.Tensor]
     com_jacobian: torch.Tensor
+
+
+class ControlledRollout(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_pd_controlled_rollout` returns, time-major [T x batch_size x n_dofs]
+    (or [T x n_dofs]): the joint angles, velocities and accelerations after each step (as
+    :meth:`DifferentiableRobotModel.compute_forward_dynamics_rollout`) and the joint torques the controller applied."""
+    q: torch.Tensor
+    qd: torch.Tensor
+    qdd: torch.Tensor
+    tau: torch.Tensor
 
 
 class DifferentiableRobotModel(torch.nn.Module):
@@ -892,6 +903,95 @@ class DifferentiableRobotModel(torch.nn.Module):
         else:
             out = engine.forward_dynamics_rollout_raw(self._topology, table, q0, qd0, f, dt, flags)
         return tuple(o[:, 0] for o in out) if squeeze else tuple(out)
+
+    def compute_pd_controlled_rollout(
+        self,
+        q0: torch.Tensor,
+        qd0: torch.Tensor,
+        q_ref: torch.Tensor,
+        kp: torch.Tensor,
+        kd: torch.Tensor,
+        dt: float,
+        qd_ref: Optional[torch.Tensor] = None,
+        f: Optional[torch.Tensor] = None,
+        effort_limit: Optional[torch.Tensor] = None,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = False,
+    ) -> ControlledRollout:
+        r"""Simulate a joint-space PD controller tracking reference trajectories: :meth:`compute_forward_dynamics_rollout`
+        with the torque of every step computed from the current state, all ``T`` steps in ONE launch
+        (``csrc/pd_rollout.cu``).  From ``(q_0, qd_0) = (q0, qd0)``, step ``t`` computes in fp32, in this order::
+
+            u = f[t] + kp * (q_ref[t] - q) + kd * (qd_ref[t] - qd)      # qd_ref / f None: zero tensors
+            u = torch.clamp(u, -effort_limit, effort_limit)             # only when effort_limit is given
+            qdd = compute_forward_dynamics(q, qd, u, include_gravity, use_damping)
+            qd = qd + dt * qdd
+            q = q + dt * qd
+
+        and the result is bit-identical to that Python loop on the same model.
+
+        Args:
+            q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
+            q_ref: reference joint angles of every step [T x batch_size x n_dofs] (or [T x n_dofs])
+            kp, kd: diagonal proportional / derivative gains, each [n_dofs] shared by every row or [batch_size x n_dofs]
+                per row (only [n_dofs] for 1-D ``q0``); one may be shared and the other per row
+            dt: step length in seconds (not differentiable)
+            qd_ref: reference joint velocities, shaped like ``q_ref``; None: zero
+            f: feed-forward joint forces, shaped like ``q_ref``; None: zero; never modified
+            effort_limit: symmetric torque limit [n_dofs], every entry > 0 (``inf`` allowed); None: no limit.
+                ``get_joint_limits()[i]["effort"]`` is a natural choice, but some shipped URDFs list 0 there.
+        Returns: :class:`ControlledRollout` ``(q, qd, qdd, tau)``, each [T x batch_size x n_dofs] (or [T x n_dofs]), with
+        ``q[t] = q_{t+1}``, ``qd[t] = qd_{t+1}``, ``qdd[t] = qdd_t`` and ``tau[t]`` the torque applied at step ``t``.
+        Differentiable w.r.t. q0, qd0, q_ref, qd_ref, f, kp, kd and every learnable link parameter (the articulated-body
+        adjoint stepped backwards in time, the clamp passing gradients where ``-effort_limit <= u <= effort_limit``); not
+        w.r.t. dt or effort_limit.  Argument errors raise ``AssertionError``."""
+        named = (("q0", q0), ("qd0", qd0), ("q_ref", q_ref), ("kp", kp), ("kd", kd), ("qd_ref", qd_ref), ("f", f),
+                 ("effort_limit", effort_limit))
+        for name, t in named:
+            if t is None and name in ("qd_ref", "f", "effort_limit"):
+                continue
+            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
+            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
+            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
+        n = self._n_dofs
+        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
+        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
+        assert q0.shape[-1] == n, f"expected {n} joints, got {q0.shape[-1]}"
+        assert q_ref.ndim == q0.ndim + 1 and q_ref.shape[1:] == q0.shape, \
+            "q_ref must be [T x batch_size x n_dofs] (or [T x n_dofs])."
+        for name, t in (("qd_ref", qd_ref), ("f", f)):
+            assert t is None or t.shape == q_ref.shape, f"{name} must have the shape of q_ref."
+        gain_shapes = ((n,),) if q0.ndim == 1 else ((n,), tuple(q0.shape))
+        for name, t in (("kp", kp), ("kd", kd)):
+            assert tuple(t.shape) in gain_shapes, f"{name} must be [n_dofs] or [batch_size x n_dofs] (got {tuple(t.shape)})"
+        if effort_limit is not None:
+            assert tuple(effort_limit.shape) == (n,), "effort_limit must be [n_dofs]."
+            # the values need a host read (a device synchronisation): done once per limit tensor and version, so a loop that
+            # passes the same limit pays it once; skipped while a CUDA graph is being captured, which forbids it
+            checked = getattr(self, "_checked_effort_limit", None)
+            if not (checked is not None and checked[0]() is effort_limit and checked[1] == effort_limit._version) \
+                    and not torch.cuda.is_current_stream_capturing():
+                assert bool((effort_limit > 0).all()), "effort_limit must be > 0 (inf allowed) and not NaN."
+                self._checked_effort_limit = (weakref.ref(effort_limit), effort_limit._version)
+        squeeze = q0.ndim == 1
+        if squeeze:
+            q0, qd0, q_ref = q0.unsqueeze(0), qd0.unsqueeze(0), q_ref.unsqueeze(1)
+            qd_ref = None if qd_ref is None else qd_ref.unsqueeze(1)
+            f = None if f is None else f.unsqueeze(1)
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        table = self._link_table()
+        dt = float(dt)
+        lim = None if effort_limit is None else effort_limit.detach()
+        if kp.shape != kd.shape:
+            # the kernel reads both gains in one layout: the shared one becomes a per-row view (its gradient is the sum of
+            # the per-row ones, through the expand's backward)
+            kp, kd = kp.expand(q0.shape), kd.expand(q0.shape)
+        diff = (table, q0, qd0, q_ref, qd_ref, f, kp, kd)
+        if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in diff):
+            out = engine.PDRolloutFunction.apply(*diff, self._topology, flags, dt, lim)
+        else:
+            out = engine.pd_rollout_raw(self._topology, table, q0, qd0, q_ref, kp, kd, dt, flags, qd_ref, f, lim)
+        return ControlledRollout(*(o[:, 0] for o in out)) if squeeze else ControlledRollout(*out)
 
     @tensor_check
     def compute_forward_dynamics_crba(

@@ -20,6 +20,8 @@
  *                                        algorithm, in one launch.
  *   drmb200_forward_dynamics_rollout     many semi-implicit Euler steps of the above in one launch (the reference
  *                                        integrates with a Python loop around compute_forward_dynamics), and its adjoint.
+ *   drmb200_pd_rollout                   the same rollout driven by a diagonal joint-space PD loop around reference
+ *                                        trajectories, in one launch, and its adjoint (the reference: a Python loop).
  *   drmb200_inverse_dynamics_derivatives / drmb200_forward_dynamics_derivatives   the Jacobians of the two above w.r.t.
  *                                        q, qd (and f), [B, n, n] each, one launch (the reference: autograd, row by row).
  *   drmb200_inverse_kinematics           Levenberg-Marquardt inverse kinematics of one link for a batch of pose targets,
@@ -287,6 +289,60 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
                                               const float* g_q, const float* g_qd, const float* g_qdd,
                                               float* q0_grad, float* qd0_grad, float* f_grad,
                                               float* table_grad, void* workspace, void* cuda_stream);
+
+/*
+ * PD-controlled rollout: drmb200_forward_dynamics_rollout with a diagonal joint-space PD law closing the loop inside the
+ * same launch.  Starting from (q_0, qd_0) = (q0, qd0), step t = 0 .. n_steps-1 computes, in fp32 and in exactly this
+ * order, every operation rounded separately (no FMA):
+ *     e_t   = q_ref[t] - q_t
+ *     ed_t  = qd_ref[t] - qd_t                          qd_ref NULL: a zero tensor (0.f - qd_t)
+ *     u_t   = (f[t] + kp * e_t) + kd * ed_t             f NULL: a zero tensor (0.f + kp * e_t); each "kp *" one rounded
+ *                                                       multiply, then a rounded add
+ *     tau_t = clamp(u_t, -effort_limit, effort_limit)   only when effort_limit is given; NaN propagates (torch.clamp)
+ *     qdd_t = FD(q_t, qd_t, tau_t)                      exactly drmb200_forward_dynamics with the same flags
+ *     qd_{t+1} = qd_t + dt * qdd_t;   q_{t+1} = q_t + dt * qd_{t+1}   as drmb200_forward_dynamics_rollout
+ * so the trajectory is bit-identical to the torch loop
+ *     u = f[t] + kp * (q_ref[t] - q) + kd * (qd_ref[t] - qd); u = clamp(u, -lim, lim);
+ *     qdd = forward_dynamics(q, qd, u); qd = qd + dt * qdd; q = q + dt * qd
+ * Layout is time-major:
+ *   q0, qd0                        [B, n_dofs]
+ *   q_ref, qd_ref, f               [n_steps, B, n_dofs]   qd_ref and f may be NULL (never modified)
+ *   kp, kd                         both [n_dofs], shared by every row (gains_per_row = 0), or both [B, n_dofs]
+ *                                  (gains_per_row = 1)
+ *   effort_limit                   [n_dofs], every entry > 0 (inf allowed), or NULL for no limit
+ *   q, qd, qdd, tau                [n_steps, B, n_dofs]   q[t] = q_{t+1}, qd[t] = qd_{t+1}, qdd[t] = qdd_t, tau[t] = tau_t;
+ *                                  qdd may be NULL
+ * No allocation, no synchronisation, graph-capturable.  Outputs must not alias inputs.  batch == 0 or n_steps == 0 is a
+ * no-op.  DRMB200_EINVAL for a NULL required pointer or a negative size; DRMB200_ELIMIT when a 32-configuration CTA needs
+ * more than 227 KB of shared memory (the message names the bytes).
+ */
+int drmb200_pd_rollout(const drmb200_topology_t* topo, const float* table,
+                       const float* q0, const float* qd0, const float* q_ref, const float* qd_ref, const float* f,
+                       const float* kp, const float* kd, int32_t gains_per_row, const float* effort_limit,
+                       int64_t batch, int32_t n_steps, float dt, uint32_t flags,
+                       float* q, float* qd, float* qdd, float* tau, void* cuda_stream);
+
+/*
+ * Adjoint of drmb200_pd_rollout.  The inputs are the forward's, plus its outputs q / qd (the step inputs of steps
+ * 1 .. n_steps-1) and tau (every step's applied torque); g_q / g_qd / g_qdd / g_tau [n_steps, B, n_dofs] are the upstream
+ * gradients of q / qd / qdd / tau (NULL = zero).  Writes q0_grad / qd0_grad [B, n_dofs], q_ref_grad / qd_ref_grad /
+ * f_grad [n_steps, B, n_dofs] and kp_grad / kd_grad PER ROW, [B, n_dofs], whichever the gains' shape (a shared gain's
+ * gradient is their sum over rows); each may be NULL.  Accumulates the table gradient of all steps into table_grad (may be
+ * NULL).  The clamp passes the gradient where -effort_limit <= u_t <= effort_limit (torch.clamp's rule), u_t recomputed
+ * bit-exactly.  Runs the analytic adjoint of drmb200_forward_dynamics_backward once per step, t = n_steps-1 .. 0, at
+ * (q_t, qd_t, tau_t), with one element-wise launch per step between them (2 n_steps + 2 launches, no atomics: bitwise
+ * reproducible).  `workspace` must hold drmb200_pd_rollout_backward_workspace_bytes(topo, batch) bytes; it does not depend
+ * on n_steps.  Outputs must not alias inputs.
+ */
+int64_t drmb200_pd_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch);
+int drmb200_pd_rollout_backward(const drmb200_topology_t* topo, const float* table,
+                                const float* q0, const float* qd0, const float* q_ref, const float* qd_ref, const float* f,
+                                const float* kp, const float* kd, int32_t gains_per_row, const float* effort_limit,
+                                int64_t batch, int32_t n_steps, float dt, uint32_t flags,
+                                const float* q, const float* qd, const float* tau,
+                                const float* g_q, const float* g_qd, const float* g_qdd, const float* g_tau,
+                                float* q0_grad, float* qd0_grad, float* q_ref_grad, float* qd_ref_grad, float* f_grad,
+                                float* kp_grad, float* kd_grad, float* table_grad, void* workspace, void* cuda_stream);
 
 /*
  * Jacobians of the dynamics, one launch each (forward-mode recursions, csrc/dynamics_derivatives.cu).  Every matrix is
