@@ -126,6 +126,9 @@ int contact_dynamics_device(const drmb200_topology_t*, int32_t, const int32_t*, 
                             const float*, const float*, int64_t, uint32_t, int32_t, float, float*, float*, uint8_t*, cudaStream_t);
 int contact_impulse_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
                            const float*, int64_t, int32_t, float, float*, float*, uint8_t*, cudaStream_t);
+int contact_rollout_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                           const float*, const float*, const float*, int64_t, int32_t, float, uint32_t, int32_t, float, float,
+                           float*, float*, float*, float*, float*, uint8_t*, cudaStream_t);
 int dynamics_regressor_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t, uint32_t,
                               float*, cudaStream_t);
 int energy_momentum_device(const drmb200_topology_t*, const float*, const float*, const float*, int64_t, float*, float*, float*,
@@ -500,6 +503,16 @@ int drmb200_contact_impulse(const drmb200_topology_t* topo, int32_t n_ee, const 
                             float regularization, float* qd_plus, float* impulse, uint8_t* solved, void* cuda_stream) {
     return drm::contact_impulse_device(topo, n_ee, ee_links, table, q, qd, velocity_ref, batch, position_only, regularization,
                                        qd_plus, impulse, solved, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_contact_rollout(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                            const float* q0, const float* qd0, const float* f, const float* target_pos,
+                            const float* target_quat, int64_t batch, int32_t n_steps, float dt, uint32_t flags,
+                            int32_t position_only, float regularization, float stabilization, float* q, float* qd, float* qdd,
+                            float* force, float* accel_ref, uint8_t* solved, void* cuda_stream) {
+    return drm::contact_rollout_device(topo, n_ee, ee_links, table, q0, qd0, f, target_pos, target_quat, batch, n_steps, dt,
+                                       flags, position_only, regularization, stabilization, q, qd, qdd, force, accel_ref,
+                                       solved, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_dynamics_regressor(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

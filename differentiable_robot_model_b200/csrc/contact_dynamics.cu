@@ -8,7 +8,8 @@
 // where qdd_free is the forward dynamics at (q, qd, f) with the call's flags.
 //
 // One thread per row, one kernel template for both modes (IMPULSE).  The row follows the operational-space kernel step by
-// step, with its device code (osd_common.cuh):
+// step, with its device code (osd_common.cuh); steps 1-5 are contact_row (contact_common.cuh), which the contact rollout
+// (contact_rollout.cu) runs for every step:
 //   1. osd_walk: J, J qd and Jdot qd;
 //   2. aba_body: qdd_free, and the q-dependent U, d, cos, sin of every link (the impulse runs it at zero velocity, zero force
 //      and without gravity -- f is not read -- and keeps only U, d, cos, sin);
@@ -26,11 +27,9 @@
 // per row at M = 48) and the joint output [n].  Outputs leave through store_transposed.
 #include <cmath>
 #include "launch.cuh"
-#include "osd_common.cuh"
+#include "contact_common.cuh"
 
 namespace drm {
-
-constexpr float CONTACT_PIVOT_MIN = 1e-5f;  // smallest pivot magnitude of the equilibrated system that counts as solved
 
 struct ContactArgs {
     const float* __restrict__ table;
@@ -67,53 +66,6 @@ struct ContactSmemLayout {
         total_floats = o;
     }
 };
-
-// Solves A x = b for one row (slot-major A [M][M] and b [M], both overwritten; x returned in b; s: M scale slots), as stated
-// in include/drm_b200.h: x = S y with (S A S) y = S b, S = diag(|A_kk|^-1/2), by Gaussian elimination with partial pivoting.
-// Returns false (b then undefined) when the row is unsolved.
-template <int T>
-__device__ __forceinline__ bool contact_solve(float* A, float* b, float* s, int M) {
-    const int rs = M * T;
-    for (int k = 0; k < M; ++k) {
-        const float d = fabsf(A[k * rs + k * T]);
-        if (!(d > 0.f) || !isfinite(d)) return false;
-        s[k * T] = 1.0f / sqrtf(d);
-    }
-    for (int i = 0; i < M; ++i) {
-        const float si = s[i * T];
-        for (int j = 0; j < M; ++j) A[i * rs + j * T] = si * A[i * rs + j * T] * s[j * T];
-        b[i * T] *= si;
-    }
-    for (int k = 0; k < M; ++k) {
-        int p = k;
-        float best = fabsf(A[k * rs + k * T]);
-        for (int i = k + 1; i < M; ++i) {               // strictly larger: ties go to the lower row
-            const float v = fabsf(A[i * rs + k * T]);
-            if (v > best) { best = v; p = i; }
-        }
-        const float piv = A[p * rs + k * T];
-        if (!(fabsf(piv) > CONTACT_PIVOT_MIN) || !isfinite(piv)) return false;
-        if (p != k) {
-            for (int j = k; j < M; ++j) {
-                const float t = A[k * rs + j * T]; A[k * rs + j * T] = A[p * rs + j * T]; A[p * rs + j * T] = t;
-            }
-            const float t = b[k * T]; b[k * T] = b[p * T]; b[p * T] = t;
-        }
-        const float inv = 1.0f / piv;
-        for (int i = k + 1; i < M; ++i) {
-            const float l = A[i * rs + k * T] * inv;
-            for (int j = k + 1; j < M; ++j) A[i * rs + j * T] = fmaf(-l, A[k * rs + j * T], A[i * rs + j * T]);
-            b[i * T] = fmaf(-l, b[k * T], b[i * T]);
-        }
-    }
-    for (int i = M - 1; i >= 0; --i) {
-        float x = b[i * T];
-        for (int j = i + 1; j < M; ++j) x = fmaf(-A[i * rs + j * T], b[j * T], x);
-        b[i * T] = x / A[i * rs + i * T];
-    }
-    for (int i = 0; i < M; ++i) b[i * T] *= s[i * T];
-    return true;
-}
 
 template <int T, bool IMPULSE>
 __global__ void __launch_bounds__(T)
@@ -165,50 +117,8 @@ contact_dynamics_kernel(const __grid_constant__ TreeProgram prog, const __grid_c
     if (bulk) mbar_wait(&mbar, 0);
 
     if (tid < valid) {
-        const float* qrow = s_q + tid * n;
-        const float* qdrow = s_qd + tid * n;
-        float* frow = s_f + tid * n;
-        float* xrow = s_qdd + tid * n;
-        const float* ref = smem + L.ref + tid * M;
-        float* lk0 = smem + L.aba.link + tid;
-        float* sl0 = smem + L.aba.slots + tid;
-        float* J = smem + L.jac + tid;
-        float* vel = smem + L.vel + tid;
-        float* bias = smem + L.bias + tid;
-        float* lam = smem + L.lam + tid;
-        float* A = smem + L.a + tid;
-        float* out = smem + L.out + tid;
-        const int rs = n_u * T;
-        osd_walk<T>(P, s_tab, qrow, qdrow, MR, J, vel, bias, smem + L.jscr + tid, smem + L.state + tid);
-        if (!IMPULSE) {
-            aba_body<T>(prog, s_tab, qrow, qdrow, frow, xrow, lk0, sl0, args.flags);
-            for (int m = 0; m < M; ++m) {           // a_ref - (J qdd_free + Jdot qd)
-                float s = bias[m * T];
-                for (int u = 0; u < n_u; ++u) s = fmaf(J[m * rs + u * T], xrow[P.u_dof[u]], s);
-                lam[m * T] = ref[m] - s;
-            }
-            for (int c = 0; c < n; ++c) out[c * T] = xrow[c];
-        } else {
-            aba_body<T>(prog, s_tab, qrow, frow, frow, xrow, lk0, sl0, 0u);
-            for (int m = 0; m < M; ++m) lam[m * T] = ref[m] - vel[m * T];     // v_ref - J qd
-            for (int c = 0; c < n; ++c) out[c * T] = qdrow[c];
-        }
-        osd_inverse_inertia<T>(prog, P, s_tab, M, J, A, frow, xrow, lk0, sl0);
-        for (int k = 0; k < M; ++k) A[(k * M + k) * T] += args.mu;
-        const bool ok = contact_solve<T>(A, lam, smem + L.scale + tid, M);
-        if (ok) {                                   // + G J^T lambda
-            for (int c = 0; c < n; ++c) frow[c] = 0.f;
-            for (int u = 0; u < n_u; ++u) {
-                float s = 0.f;
-                for (int m = 0; m < M; ++m) s = fmaf(J[m * rs + u * T], lam[m * T], s);
-                frow[P.u_dof[u]] = s;
-            }
-            aba_unit_response<T>(prog, s_tab, frow, xrow, lk0, sl0);
-            for (int c = 0; c < n; ++c) out[c * T] += xrow[c];
-        } else {
-            for (int c = 0; c < n; ++c) out[c * T] = __int_as_float(0x7fc00000);
-            for (int m = 0; m < M; ++m) lam[m * T] = __int_as_float(0x7fc00000);
-        }
+        bool ok;
+        DRM_CONTACT_ROW(T, IMPULSE, false, nullptr, args.flags, args.mu, ok, );
         args.solved[tile_start + tid] = ok ? 1 : 0;
     }
     __syncthreads();
@@ -252,8 +162,9 @@ static int contact_launch(const TreeProgram& prog, const UnionProgram& P, const 
 #undef DRM_LAUNCH_CONTACT
 }
 
-// The argument checks shared by both entry points; on success P and *prog describe the walk and the (unfolded) tree.
-static int contact_programs(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, float regularization,
+// The argument checks shared by both entry points and the contact rollout (contact_rollout.cu); on success P and *prog
+// describe the walk and the (unfolded) tree.
+int contact_programs(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, float regularization,
                             int64_t batch, UnionProgram* P, const TreeProgram** prog) {
     if (n_ee < 1 || n_ee > MT_MAX_EE) { set_error("n_ee=%d outside [1, %d]", n_ee, MT_MAX_EE); return DRMB200_EINVAL; }
     if (ee_links == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }

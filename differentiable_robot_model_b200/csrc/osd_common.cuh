@@ -1,5 +1,5 @@
-// osd_common.cuh -- the per-row pieces of the operational-space dynamics, shared by operational_space.cu and
-// contact_dynamics.cu so that the two compute J, Jdot qd and J G J^T with the same arithmetic:
+// osd_common.cuh -- the per-row pieces of the operational-space dynamics, shared by operational_space.cu,
+// contact_dynamics.cu and contact_rollout.cu so that they compute J, Jdot qd and J G J^T with the same arithmetic:
 //   osd_walk              the kinematic walk of the union of the root -> link paths: J, J qd and Jdot qd
 //   aba_unit_response     x = G tau, on the articulated inertias aba_body left behind (two O(n) sweeps)
 //   osd_inverse_inertia   J G J^T, formed in the smaller of the two spaces
@@ -14,9 +14,10 @@ constexpr int OSD_STATE = 24;          // floats of a spilled branch state: R (9
 
 // The kinematic walk of one row: J [M][n_u], velocity and bias [M] (this row's slot-major slots; entries of links that are
 // not walked -- the root -- and of joints off a link's path are left as staged: zero).  qrow / qdrow: the row's q, qd.
-template <int T>
+// POSES: also every link's world pose, p (3) then R (9, row-major, canonical +z frame) at pose + 12 l T.
+template <int T, bool POSES = false>
 __device__ __forceinline__ void osd_walk(const UnionProgram& P, const float* s_tab, const float* qrow, const float* qdrow, int MR,
-                                         float* J, float* vel, float* bias, float* jscr, float* st) {
+                                         float* J, float* vel, float* bias, float* jscr, float* st, float* pose = nullptr) {
     const MultiProgram& W = P.walk;
     const V3 zero = v3(0.f, 0.f, 0.f);
     M3 R = identity3();
@@ -63,6 +64,7 @@ __device__ __forceinline__ void osd_walk(const UnionProgram& P, const float* s_t
         stv(vel + MR * l * T, T, v);
         stv(bias + MR * l * T, T, a);
         if (MR == 6) { stv(vel + (MR * l + 3) * T, T, w); stv(bias + (MR * l + 3) * T, T, A); }
+        if (POSES) { float* ps = pose + 12 * l * T; stv(ps, T, p); stm(ps + 3 * T, T, R); }
     }
 }
 

@@ -121,6 +121,11 @@ _SIGNATURES = {
     "drmb200_contact_impulse": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
                                                _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int32,
                                                ctypes.c_float, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_contact_rollout": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                               _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                               ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_uint32, ctypes.c_int32,
+                                               ctypes.c_float, ctypes.c_float, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                               _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
     "drmb200_dynamics_regressor": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                   ctypes.c_int64, ctypes.c_uint32, _c_float_p, ctypes.c_void_p]),
     "drmb200_energy_momentum": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64,
@@ -582,6 +587,36 @@ def contact_impulse_raw(topo, ee_links, table, q, qd, velocity_ref=None, positio
                                            _ptr(impulse), _ptr(solved), _stream())
     _check(rc, "drmb200_contact_impulse")
     return qd_plus, impulse, solved.view(torch.bool)
+
+
+def contact_rollout_raw(topo, ee_links, table, q0, qd0, f, dt, flags, target_pos=None, target_quat=None, position_only=False,
+                        regularization=0.0, stabilization=0.0, want_qdd=True, want_force=True, want_accel_ref=False):
+    """(q, qd, qdd [T, B, n], force [T, B, M], accel_ref [T, B, M], solved [B] bool) of T semi-implicit Euler steps of the
+    contact dynamics at the links `ee_links` with Baumgarte rate `stabilization`, one launch (drmb200_contact_rollout).
+    f [T, B, n]; target_pos [n_ee, B, 3] / target_quat [n_ee, B, 4] or None (the poses at q0).  qdd / force / accel_ref are
+    None unless wanted."""
+    _require_cuda(table, q0, qd0, f, target_pos, target_quat)
+    q0, qd0, f = q0.contiguous(), qd0.contiguous(), f.contiguous()
+    target_pos = None if target_pos is None else target_pos.contiguous()
+    target_quat = None if target_quat is None else target_quat.contiguous()
+    T, B, n = f.shape
+    E = len(ee_links)
+    M = (3 if position_only else 6) * E
+    dev = q0.device
+    q, qd = (torch.empty((T, B, n), device=dev, dtype=torch.float32) for _ in range(2))
+    qdd = torch.empty((T, B, n), device=dev, dtype=torch.float32) if want_qdd else None
+    force = torch.empty((T, B, M), device=dev, dtype=torch.float32) if want_force else None
+    accel_ref = torch.empty((T, B, M), device=dev, dtype=torch.float32) if want_accel_ref else None
+    solved = torch.empty(B, device=dev, dtype=torch.uint8)
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    with _on(dev):
+        rc = lib().drmb200_contact_rollout(ctypes.byref(topo), E, links, _ptr(table), _ptr(q0), _ptr(qd0), _ptr(f),
+                                           _ptr(target_pos), _ptr(target_quat), B, T, ctypes.c_float(dt), flags & 3,
+                                           1 if position_only else 0, ctypes.c_float(regularization),
+                                           ctypes.c_float(stabilization), _ptr(q), _ptr(qd), _ptr(qdd), _ptr(force),
+                                           _ptr(accel_ref), _ptr(solved), _stream())
+    _check(rc, "drmb200_contact_rollout")
+    return q, qd, qdd, force, accel_ref, solved.view(torch.bool)
 
 
 def kinematic_state_raw(topo, table, q, qd=None, want_poses=True, want_quats=False):

@@ -146,6 +146,18 @@ class ControlledRollout(NamedTuple):
     tau: torch.Tensor
 
 
+class ContactRollout(NamedTuple):
+    """What :meth:`DifferentiableRobotModel.compute_contact_rollout` returns, time-major: the joint angles, velocities and
+    accelerations after each step [T x batch_size x n_dofs] (as :meth:`DifferentiableRobotModel.compute_forward_dynamics_rollout`),
+    the contact forces of each step [T x batch_size x M] (laid out like :class:`ContactDynamics`'s force) and whether every
+    step of the row was solved [batch_size]."""
+    q: torch.Tensor
+    qd: torch.Tensor
+    qdd: torch.Tensor
+    force: torch.Tensor
+    solved: torch.Tensor
+
+
 class DifferentiableRobotModel(torch.nn.Module):
     """Batched rigid-body kinematics / dynamics of a URDF robot on one GPU (H100, sm_90a)."""
 
@@ -903,6 +915,92 @@ class DifferentiableRobotModel(torch.nn.Module):
         else:
             out = engine.forward_dynamics_rollout_raw(self._topology, table, q0, qd0, f, dt, flags)
         return tuple(o[:, 0] for o in out) if squeeze else tuple(out)
+
+    def compute_contact_rollout(
+        self,
+        q0: torch.Tensor,
+        qd0: torch.Tensor,
+        f: torch.Tensor,
+        link_names: List[str],
+        dt: float,
+        target_pos: Optional[torch.Tensor] = None,
+        target_quat: Optional[torch.Tensor] = None,
+        stabilization: float = 0.0,
+        include_gravity: Optional[bool] = True,
+        use_damping: Optional[bool] = False,
+        position_only: bool = False,
+        regularization: float = 0.0,
+    ) -> ContactRollout:
+        r"""Simulate the links held by bilateral rigid contacts: :meth:`compute_contact_dynamics` integrated over ``T`` steps
+        of semi-implicit Euler, with Baumgarte stabilisation towards fixed targets, all in ONE launch
+        (``csrc/contact_rollout.cu``; stated in ``include/drm_b200.h``).  From ``(q, qd) = (q0, qd0)``, step ``t`` computes in
+        fp32, in this order, with ``p, R`` the links' poses and ``J`` their stacked Jacobians at ``q``, ``w = stabilization``::
+
+            e = p - target_pos  (and, in pose mode, the world-frame rotation vector of R R_target^T)
+            a_ref = -(2 * w) * (J qd) - (w * w) * e                        # w = 0: a_ref = 0, no term formed
+            qdd, force, ok = compute_contact_dynamics(q, qd, f[t], link_names, a_ref, ...)
+            qd = qd + dt * qdd
+            q = q + dt * qd
+
+        With ``stabilization = 0`` the result is bit-identical to that Python loop with ``accel_ref = None``.  Without
+        stabilisation the integrator's drift off the constraint accumulates; ``w * dt`` of about 0.2 is a good working choice
+        (``examples/pinned_end_effector_iiwa.py`` holds the Kuka end effector within a fraction of a millimetre with it).
+        With ``use_damping`` the joints' damping torque ``-d qd`` enters each step at the current ``qd``, so the integrate is
+        explicit in it and stable only for ``dt`` below about ``2 I / d`` (``I`` a joint's effective inertia): the Allegro
+        hand's fingers (damping 3-8 N m s/rad on links of a few grams) diverge within ten steps at ``dt = 1e-3`` and at
+        ``1e-4``; simulate them without damping or at a far smaller step.
+
+        Args:
+            q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
+            f: applied joint forces of every step [T x batch_size x n_dofs] (or [T x n_dofs])
+            link_names: the held links (at most 8, distinct), stacked in this order; each needs a movable joint on its
+                root path
+            dt: step length in seconds
+            target_pos: where each link's origin is held [n_links x batch_size x 3] (``[n_links x 3]`` for 1-D ``q0``);
+                None: the links' poses at ``q0``
+            target_quat: in pose mode, each link's held orientation [n_links x batch_size x 4] xyzw (normalised here),
+                given together with ``target_pos``; must be None with ``position_only``
+            stabilization: the Baumgarte rate ``w >= 0`` [1/s]
+            include_gravity, use_damping, position_only, regularization: as for :meth:`compute_contact_dynamics`
+        Returns: :class:`ContactRollout` ``(q, qd, qdd, force, solved)`` with ``q[t] = q_{t+1}``, ``qd[t] = qd_{t+1}``,
+        ``qdd[t] = qdd_t`` and ``force[t]`` the contact forces of step ``t``; the batch dimension is dropped for 1-D inputs.
+        ``solved`` is False for a row where some step was not solved; that step and every later one of the row are NaN.
+        The outputs carry no autograd graph: they use the current values of the link parameters (learnable and fused ones
+        included) but are not differentiable.  Argument errors raise ``AssertionError``."""
+        links = self._contact_links(link_names)
+        E = len(links)
+        for name, t in (("q0", q0), ("qd0", qd0), ("f", f), ("target_pos", target_pos), ("target_quat", target_quat)):
+            if t is None and name.startswith("target"):
+                continue
+            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
+            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
+            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
+        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
+        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
+        assert q0.shape[-1] == self._n_dofs, f"expected {self._n_dofs} joints, got {q0.shape[-1]}"
+        assert f.ndim == q0.ndim + 1 and f.shape[1:] == q0.shape, "f must be [T x batch_size x n_dofs] (or [T x n_dofs])."
+        if position_only:
+            assert target_quat is None, "target_quat must be None with position_only"
+        else:
+            assert (target_pos is None) == (target_quat is None), "give target_pos and target_quat together in pose mode"
+        stabilization = float(stabilization)
+        assert stabilization >= 0 and stabilization != float("inf"), "stabilization must be finite and >= 0"
+        squeeze = q0.ndim == 1
+        if squeeze:
+            q0, qd0, f = q0.unsqueeze(0), qd0.unsqueeze(0), f.unsqueeze(1)
+            target_pos = None if target_pos is None else target_pos.unsqueeze(1)
+            target_quat = None if target_quat is None else target_quat.unsqueeze(1)
+        B = q0.shape[0]
+        assert target_pos is None or tuple(target_pos.shape) == (E, B, 3), "target_pos must be [n_links x batch_size x 3]"
+        assert target_quat is None or tuple(target_quat.shape) == (E, B, 4), "target_quat must be [n_links x batch_size x 4]"
+        flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        q, qd, qdd, force, _, solved = engine.contact_rollout_raw(
+            self._topology, links, self._link_table().detach(), q0.detach(), qd0.detach(), f.detach(), float(dt), flags,
+            None if target_pos is None else target_pos.detach(), None if target_quat is None else target_quat.detach(),
+            bool(position_only), float(regularization), stabilization)
+        if squeeze:
+            return ContactRollout(q[:, 0], qd[:, 0], qdd[:, 0], force[:, 0], solved[0])
+        return ContactRollout(q, qd, qdd, force, solved)
 
     def compute_pd_controlled_rollout(
         self,

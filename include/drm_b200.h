@@ -32,6 +32,8 @@
  *   drmb200_contact_dynamics / drmb200_contact_impulse   joint accelerations and contact forces under rigid contacts at
  *                                        several links, and the joint velocities and impulses of an impact there, one launch
  *                                        each (the reference has none of these).
+ *   drmb200_contact_rollout              T semi-implicit Euler steps of the contact dynamics with Baumgarte stabilisation
+ *                                        towards fixed link targets, one launch (the reference has none of these).
  *   drmb200_dynamics_regressor           the joint-torque regressor Y, tau = Y . (I_o, mc, m, damping of every link), one
  *                                        launch (the reference: autograd of compute_inverse_dynamics, row by row).
  *   drmb200_energy_momentum              kinetic and potential energy, generalized momentum H(q) qd, centre of mass, its
@@ -514,6 +516,40 @@ int drmb200_contact_impulse(const drmb200_topology_t* topo, int32_t n_ee, const 
                             const float* q, const float* qd, const float* velocity_ref, int64_t batch,
                             int32_t position_only, float regularization,
                             float* qd_plus, float* impulse, uint8_t* solved, void* cuda_stream);
+
+/*
+ * Contact-constrained rollouts: T steps of semi-implicit Euler over drmb200_contact_dynamics with Baumgarte stabilisation,
+ * ONE launch (csrc/contact_rollout.cu).  The links ee_links [n_ee] (host array, 1 <= n_ee <= 8), position_only, M = 3 n_ee or
+ * 6 n_ee, mu = regularization >= 0 and the flags (DRMB200_GRAVITY, DRMB200_DAMPING) are those of drmb200_contact_dynamics;
+ * dt is the step and omega = stabilization >= 0 (finite) the stabilisation rate.  Targets per link and row: a position p*
+ * and, in pose mode, an orientation quat* (xyzw, normalised in the kernel as the IK kernels do); when none are given they
+ * are the links' poses at q0, taken from the kernel's own walk at step 0.
+ * From (q_0, qd_0) = (q0, qd0), step t = 0 ... T-1, in fp32:
+ *   1. walk at (q_t, qd_t) as drmb200_operational_space_dynamics does: J, v = J qd, Jdot qd and every link's pose (p_l, R_l);
+ *   2. e [M]: per link p_l - p*_l and, in pose mode, the world-frame rotation vector of R_l R*_l^T, the shorter way round
+ *      (minus the rotation error of drmb200_inverse_kinematics, so that de/dt ~ omega_l, the angular rows of J qd);
+ *   3. a_ref = -(2 omega) v - (omega^2) e, with 2 omega and omega^2 each rounded once, every product and the difference
+ *      rounded once; omega == 0 forms no term: a_ref = 0 exactly and the step is drmb200_contact_dynamics(accel_ref = NULL);
+ *   4. (qdd_t, lambda_t, ok_t) = drmb200_contact_dynamics(q_t, qd_t, f[t], a_ref), the same device code in the same order;
+ *   5. qd_{t+1} = qd_t + dt * qdd_t;  q_{t+1} = q_t + dt * qd_{t+1}, every product and sum rounded separately.
+ * With DRMB200_DAMPING the damping torque -d qd_t enters qdd_t explicitly, so the integrate is stable only for dt below
+ * about 2 I / d (I a joint's effective inertia); light, strongly damped links need a far smaller step (the Allegro
+ * fingers diverge within ten steps at dt = 1 ms and at 0.1 ms).
+ * Outputs, time-major, caller-allocated, must not alias inputs: q [T, B, n] (q[t] = q_{t+1}), qd [T, B, n], qdd [T, B, n]
+ * (qdd_t) or NULL, force [T, B, M] (lambda_t) or NULL, accel_ref [T, B, M] (the a_ref of step t) or NULL, solved [B] uint8
+ * (the AND of ok_t over all steps).  An unsolved step gives NaN in qdd and lambda, so the row's state is NaN from then on;
+ * other rows are unaffected.  Inputs: q0, qd0 [B, n], f [T, B, n] (required), target_pos [n_ee, B, 3] and, in pose mode,
+ * target_quat [n_ee, B, 4] (both or neither; NULL in position mode), table; device pointers.  No allocation, no
+ * synchronisation (graph-capturable).  batch == 0 or n_steps == 0 is a no-op (no launch).  DRMB200_EINVAL for the argument
+ * errors of drmb200_contact_dynamics, n_steps < 0, a negative or non-finite stabilization, a target_quat in position mode
+ * or only one of the two targets in pose mode; DRMB200_ELIMIT for more live branch points than the forward-dynamics kernel
+ * handles or, naming the bytes, when a one-row CTA needs more than 227 KB of shared memory.
+ */
+int drmb200_contact_rollout(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                            const float* q0, const float* qd0, const float* f, const float* target_pos,
+                            const float* target_quat, int64_t batch, int32_t n_steps, float dt, uint32_t flags,
+                            int32_t position_only, float regularization, float stabilization, float* q, float* qd, float* qdd,
+                            float* force, float* accel_ref, uint8_t* solved, void* cuda_stream);
 
 /*
  * The joint-torque regressor of the inertial parameters and dampings, one launch (csrc/dynamics_regressor.cu).  tau is
