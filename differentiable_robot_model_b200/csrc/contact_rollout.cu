@@ -14,21 +14,21 @@
 // none are given, taken from the step-0 walk: p*_l = p_l(q0) and quat*_l = the quaternion of R_l(q0), un-permuted as
 // drmb200_fk_jacobian returns it, so both kinds go through rotvec_error.
 //
-// Mapping: the contact kernel's (one thread per row, T rows per CTA, the same slot-major row state) with the rollout's time
-// loop (rollout.cu).  Once per CTA the canonical (unfolded) table, the (q0, qd0) tile and the targets are staged; the state
-// then lives in shared memory for all steps.  Per step the f_t tile arrives by TMA bulk copy into a double buffer (f_{t+1}
-// is issued before step t computes; two mbarriers, phase parity t / 2) and is copied into the ABA's f row, which the
-// unit-response sweeps overwrite.  q / qd leave as bulk stores straight from the state rows, so thread 0 waits for the
-// previous step's store READS only right before the next integrate; qdd is copied from the slot-major output into a
-// row-major double buffer and leaves by bulk store too.  lambda (slot-major) leaves through store_transposed and a_ref
-// (row-major, the layout the contact row reads) through a linear cooperative copy.  Tiles whose size or base is not 16-byte
-// aligned take cooperative copies.  The solved flag is the AND of every step's, kept in a register and written once.
+// Mapping: the contact kernel's (one thread per row, T rows per CTA, the same slot-major row state) with the rollouts' time
+// loop (rollout_pipeline.cuh: state staging, f double buffer, integrate and q / qd / qdd stores).  Once per CTA the
+// canonical (unfolded) table, the (q0, qd0) tile and the targets are staged; the state then lives in shared memory for all
+// steps.  Per step the f_t tile is copied into the ABA's f row, which the unit-response sweeps overwrite; the integrate
+// reads qdd from the slot-major output, which is also copied into a row-major double buffer for the pipeline's qdd store.
+// lambda (slot-major) leaves through store_transposed and a_ref (row-major, the layout the contact row reads) through a
+// linear cooperative copy, after the pipeline's stores.  The solved flag is the AND of every step's, kept in a register
+// and written once.
 //
 // Algorithmic HBM bytes per configuration-step: f in 4n, q / qd / qdd out 12n, force out 4M (a_ref 4M more when asked for).
 #include <cmath>
 #include "contact_common.cuh"
 #include "ik_common.cuh"
 #include "launch.cuh"
+#include "rollout_pipeline.cuh"
 
 namespace drm {
 
@@ -105,33 +105,14 @@ contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_co
     float* s_f = smem + L.aba.f;
     float* s_qdd = smem + L.aba.qdd;
     float* s_tab = smem + L.aba.table;
-    float* s_fb = smem + L.fbuf;
     float* s_qddb = smem + L.qddbuf;
-
     const int tid = threadIdx.x;
     const int64_t tile_start = (int64_t)blockIdx.x * T;
-    const int64_t tile_off = tile_start * n;
-    const int valid = (int)min((int64_t)T, args.batch - tile_start);
-    const int tile_floats = valid * n;
-    const int64_t step = args.batch * n;                 // floats between the [B, n] slices of consecutive steps
-    const bool vec_ok = args.aligned;
-    const bool bulk = args.aligned && ((tile_floats & 3) == 0);
-    const uint32_t bytes = (uint32_t)tile_floats * 4u;
 
-    if (bulk) {
-        if (tid == 0) {
-            mbar_init(&mbar[0], 1);
-            mbar_init(&mbar[1], 1);
-            fence_mbar_init();
-            mbar_arrive_expect_tx(&mbar[0], 3u * bytes);
-            bulk_g2s(s_q, args.q0 + tile_off, bytes, &mbar[0]);
-            bulk_g2s(s_qd, args.qd0 + tile_off, bytes, &mbar[0]);
-            bulk_g2s(s_fb, args.f + tile_off, bytes, &mbar[0]);
-        }
-    } else {
-        coop_copy(s_q, args.q0 + tile_off, tile_floats, vec_ok);
-        coop_copy(s_qd, args.qd0 + tile_off, tile_floats, vec_ok);
-    }
+    const RolloutPipeline<T> pipe(mbar, s_q, s_qd, smem + L.fbuf, args.f, nullptr, nullptr, args.q, args.qd, n, args.batch,
+                                  args.n_steps, args.dt, args.aligned);
+    const int valid = pipe.valid;
+    pipe.begin(args.q0, args.qd0);
     stage_canonical_table(s_tab, args.table, prog, T);
     // J, velocity and bias start at zero (columns off a link's path); a_ref stays zero without stabilisation
     for (int i = L.ref + tid; i < L.jscr; i += T) smem[i] = 0.f;
@@ -153,24 +134,9 @@ contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_co
         for (int l = 0; l < E; ++l) normalize_target_quat(smem + L.tquat + 4 * l * T + tid, T);
 
     uint8_t solved = 1;
-    const float dt = args.dt;
     for (int t = 0; t < args.n_steps; ++t) {
-        const int b = t & 1;
-        float* s_ft = s_fb + b * T * n;
-        float* s_qddt = s_qddb + b * T * n;
-        if (bulk) {
-            // buffer b ^ 1 was last read by the f-row copy of step t - 1, which every thread finished (and fenced against
-            // the async proxy) before the barrier that ended step t - 1
-            if (tid == 0 && t + 1 < args.n_steps) {
-                mbar_arrive_expect_tx(&mbar[b ^ 1], bytes);
-                bulk_g2s(s_fb + (b ^ 1) * T * n, args.f + (t + 1) * step + tile_off, bytes, &mbar[b ^ 1]);
-            }
-            mbar_wait(&mbar[b], (uint32_t)(t >> 1) & 1u);
-        } else {
-            coop_copy(s_ft, args.f + t * step + tile_off, tile_floats, vec_ok);
-            __syncthreads();
-        }
-
+        const float* s_ft = pipe.fetch(t);
+        float* s_qddt = s_qddb + (t & 1) * T * n;
         if (tid < valid) {
             for (int c = 0; c < n; ++c) s_f[tid * n + c] = s_ft[tid * n + c];
             // steps 2-3, between the walk and the contact dynamics: the targets (step 0, when not given) and a_ref
@@ -213,36 +179,7 @@ contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_co
                 for (int c = 0; c < n; ++c) s_qddt[tid * n + c] = smem[L.out + c * T + tid];
         }
 
-        if (bulk) {
-            if (tid == 0) bulk_wait_read<0>();           // the stores of step t - 1 have read s_q / s_qd
-            __syncthreads();
-        }
-        if (tid < valid) {
-            float* qr = s_q + tid * n;
-            float* qdr = s_qd + tid * n;
-            const float* ar = smem + L.out + tid;
-            for (int k = 0; k < n; ++k) {
-                const float v = __fadd_rn(qdr[k], __fmul_rn(dt, ar[k * T]));
-                qdr[k] = v;
-                qr[k] = __fadd_rn(qr[k], __fmul_rn(dt, v));
-            }
-        }
-        if (bulk) {
-            fence_proxy_async();
-            __syncthreads();
-            if (tid == 0) {
-                bulk_s2g(args.q + t * step + tile_off, s_q, bytes);
-                bulk_s2g(args.qd + t * step + tile_off, s_qd, bytes);
-                if (args.qdd != nullptr) bulk_s2g(args.qdd + t * step + tile_off, s_qddt, bytes);
-                bulk_commit();
-            }
-        } else {
-            __syncthreads();
-            coop_copy(args.q + t * step + tile_off, s_q, tile_floats, vec_ok);
-            coop_copy(args.qd + t * step + tile_off, s_qd, tile_floats, vec_ok);
-            if (args.qdd != nullptr) coop_copy(args.qdd + t * step + tile_off, s_qddt, tile_floats, vec_ok);
-            // the next step's integrate rewrites s_q / s_qd only after the barrier that follows its f copy
-        }
+        pipe.integrate_and_store(t, smem + L.out + tid, T, args.qdd, s_qddt);     // q̈ from the slot-major output
         const int64_t mrow = ((int64_t)t * args.batch + tile_start) * M;
         if (args.force != nullptr) store_transposed(args.force + mrow, smem + L.lam, M, valid, T);
         if (args.accel_ref != nullptr) {
@@ -251,7 +188,7 @@ contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_co
         }
         if (args.force != nullptr || args.accel_ref != nullptr) __syncthreads();    // before the next step rewrites them
     }
-    if (bulk && tid == 0) bulk_wait_read<0>();
+    pipe.finish();
     if (tid < valid) args.solved[tile_start + tid] = solved;
 }
 

@@ -13,6 +13,9 @@ namespace drm {
 constexpr size_t SMEM_TWO_CTAS = 113 * 1024;    // a CTA at most this large leaves room for a second one on the SM
 constexpr size_t SMEM_CTA_MAX = 227 * 1024;     // the most shared memory one CTA may have
 
+// bytes rounded up to a multiple of 256: the alignment of every slice a wrapper carves out of a caller's workspace
+inline int64_t round256(int64_t bytes) { return (bytes + 255) & ~(int64_t)255; }
+
 // every pointer 16-byte aligned (float4 and TMA bulk copies); a null pointer counts as aligned
 template <typename... P>
 inline bool aligned16(const P*... p) { return (((reinterpret_cast<uintptr_t>(p) & 15u) == 0) && ...); }

@@ -1,20 +1,24 @@
 // rollout.cu -- batched forward-dynamics rollouts (sm_90a): T steps of semi-implicit Euler over the articulated-body
-// algorithm in ONE launch, and the reverse-time adjoint of the same rollout.
+// algorithm in ONE launch, open loop or with a diagonal joint-space PD law closing the loop, and the reverse-time adjoint
+// of both.
 //
-// Step t, fp32, in exactly this order (qdd_t is what drmb200_forward_dynamics returns for (q_t, qd_t, f_t)):
+// Open-loop step t, fp32, in exactly this order (qdd_t is what drmb200_forward_dynamics returns for (q_t, qd_t, f_t)):
 //   qdd_t = FD(q_t, qd_t, f_t);   qd_{t+1} = qd_t + dt * qdd_t;   q_{t+1} = q_t + dt * qd_{t+1}
-// each "+ dt *" one rounded multiply and one rounded add (__fmul_rn / __fadd_rn, never contracted to an FMA), so that the
-// trajectory is bit-identical to a loop of forward-dynamics launches followed by `qd = qd + dt * qdd; q = q + dt * qd`.
+// PD step t, every operation rounded separately (the definition is stated in include/drm_b200.h):
+//   e_t = q_ref[t] - q_t;  ed_t = qd_ref[t] - qd_t;  u_t = (f[t] + kp e_t) + kd ed_t;  tau_t = clamp(u_t, -lim, lim)
+//   qdd_t = FD(q_t, qd_t, tau_t), then the same integrate.  (qd_ref / f absent: 0 - qd_t / 0 + kp e_t; lim absent: no
+//   clamp.)
+// each "+ dt *" one rounded multiply and one rounded add, so that the trajectory is bit-identical to the stepwise torch loop.
 //
 // Forward mapping: the articulated-body kernel's (aba.cu) -- one thread per configuration, T per CTA, the same per-thread
-// body (aba_body.cuh) -- with a time loop inside.  Once per CTA the table is staged (and folded, "rnea_fold") and the
-// (q0, qd0) tile loaded; the state then lives in shared memory for all steps.  Per step the f_t tile arrives by TMA bulk
-// copy into a double buffer (f_{t+1} is issued before step t computes; two mbarriers, phase parity t / 2), and the q / qd /
-// qdd tiles of step t leave as bulk stores.  s_q / s_qd are both the live state and the store source, so thread 0 waits for
-// the previous store's READS only right before the next integrate: the store drains while the next step's passes run.  qdd
-// is double-buffered for the same reason.  Tiles whose size or base is not 16-byte aligned take cooperative copies.
-//
-// Algorithmic HBM bytes per configuration-step: f in 4n, q / qd / qdd out 12n = 16n (112 B at n = 7; 12n without qdd).
+// body (aba_body.cuh) -- with the time loop of rollout_pipeline.cuh inside (rollout_kernel: its own copy).  Once per CTA the table is staged (and folded,
+// "rnea_fold") and the (q0, qd0) tile loaded; the state then lives in shared memory for all steps.  Per step the input
+// tiles (f, or q_ref | qd_ref | f) arrive by TMA into a double buffer and q / qd / qdd (and tau) leave by bulk store; qdd
+// and tau are double-buffered.  rollout_kernel's ABA reads f straight from the input buffer.  pd_rollout_kernel stages
+// per-row gains once per CTA, shared gains and limits once as [n] rows, and each thread forms its tau_t row from the live
+// s_q / s_qd into the tau tile, which aba_body reads as its f.
+// Algorithmic HBM bytes per configuration-step: open loop f in 4n, q / qd / qdd out 12n = 16n (112 B at n = 7; 12n without
+// qdd); PD q_ref 4n (+ qd_ref 4n, + f 4n) in, q / qd / qdd / tau 16n out: up to 28n.
 //
 // Adjoint (drmb200_forward_dynamics_rollout_backward): a host loop t = T-1 ... 0 over the analytic ABA adjoint
 // (backward_aba.cu), with running adjoints a_q, a_qd of the state (start at zero):
@@ -23,14 +27,34 @@
 // and q0_grad = a_q, qd0_grad = a_qd at the end.  One element-wise launch per step fuses the post-update of step t+1 with
 // the pre-update of step t; the table gradient of all steps is summed in the adjoint's per-CTA partial tables and reduced
 // once, so a backward is 2T + 2 launches.
+// drmb200_pd_rollout_backward folds the feedback into the same element-wise step.  With gu_t = mask_t (gf_t + g_tau[t]),
+// mask_t = (-lim <= u_t <= lim) (1 without a limit; u_t recomputed bit-exactly), the post-update of step t becomes
+//   a_q = (a_q + gq) - kp gu_t;  a_qd = (a_qd' + gqd) - kd gu_t;  f_grad[t] = gu_t;  q_ref_grad[t] = kp gu_t;
+//   qd_ref_grad[t] = kd gu_t;  kp_grad += gu_t e_t;  kd_grad += gu_t ed_t      (kp_grad / kd_grad per row, [B, n])
+// still 2T + 2 launches, no atomics.
 #include "aba_body.cuh"
 #include "launch.cuh"
+#include "rollout_pipeline.cuh"
 
 namespace drm {
 
 int forward_dynamics_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
                                      uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t, bool, bool);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
+
+// u = (f + kp e) + kd ed with e = q_ref - q, ed = qd_ref - qd: the rounding of the torch expression
+// `f + kp * (q_ref - q) + kd * (qd_ref - qd)`; pass 0.f for an absent f / qd_ref (a zero tensor, -0 included)
+__device__ __forceinline__ float pd_command(float q_ref, float q, float qd_ref, float qd, float f, float kp, float kd,
+                                            float& e, float& ed) {
+    e = __fsub_rn(q_ref, q);
+    ed = __fsub_rn(qd_ref, qd);
+    return __fadd_rn(__fadd_rn(f, __fmul_rn(kp, e)), __fmul_rn(kd, ed));
+}
+
+// torch.clamp(u, -lim, lim): NaN propagates
+__device__ __forceinline__ float pd_clamp(float u, float lim) {
+    return isnan(u) ? u : fminf(fmaxf(u, -lim), lim);
+}
 
 struct RolloutArgs {
     const float* __restrict__ table;
@@ -62,6 +86,9 @@ struct RolloutSmem {
     }
 };
 
+// The open-loop kernel keeps its own copy of rollout_pipeline.cuh's time loop: built on RolloutPipeline it compiled to a
+// different schedule of the ABA body (same registers and stack) that measured 1.5-2.5 % slower on an H100 80GB HBM3 at
+// 700 W (DESIGN.md §5), while the PD and contact kernels ran as fast as before.  Its ordering is the pipeline's.
 template <int T>
 __global__ void __launch_bounds__(T)
 rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const RolloutArgs args) {
@@ -162,15 +189,139 @@ rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__
     if (bulk && tid == 0) bulk_wait_read<0>();
 }
 
+struct PDRolloutArgs {
+    const float* __restrict__ table;
+    const float* __restrict__ q0;
+    const float* __restrict__ qd0;
+    const float* __restrict__ q_ref;
+    const float* __restrict__ qd_ref;   // may be null
+    const float* __restrict__ f;        // may be null
+    const float* __restrict__ kp;       // [n] or [B, n]
+    const float* __restrict__ kd;
+    const float* __restrict__ lim;      // [n], may be null
+    float* __restrict__ q;
+    float* __restrict__ qd;
+    float* __restrict__ qdd;            // may be null
+    float* __restrict__ tau;
+    int64_t batch;
+    int32_t n_steps;
+    float dt;
+    uint32_t flags;
+    int32_t per_row;                    // kp / kd are [B, n]
+    int32_t aligned;                    // as RolloutArgs, over every tile pointer (and kp / kd when per row)
+};
+
+struct PDRolloutSmem {
+    int q, qd, in, tau, qdd, kp, kd, lim, table, link, slots, total_floats;
+    // n_in input tiles per step (q_ref, then qd_ref and f when given); every region starts 16-byte aligned
+    __host__ __device__ PDRolloutSmem(int T, int n, int n_links, int n_slots, int n_in, bool per_row) {
+        const int gain = ((per_row ? T : 1) * n + 3) & ~3;
+        int o = 0;
+        q = o;   o += T * n;
+        qd = o;  o += T * n;
+        in = o;  o += 2 * n_in * T * n;  // double buffer
+        tau = o; o += 2 * T * n;         // double buffer
+        qdd = o; o += 2 * T * n;         // double buffer
+        kp = o;  o += gain;
+        kd = o;  o += gain;
+        lim = o; o += (n + 3) & ~3;
+        table = o; o += n_links * DRMB200_TABLE_STRIDE;
+        link = o;  o += n_links * ABA_LINK * T;
+        slots = o; o += n_slots * ABA_SLOT * T;
+        total_floats = o;
+    }
+};
+
+template <int T>
+__global__ void __launch_bounds__(T)
+pd_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const PDRolloutArgs args) {
+    extern __shared__ __align__(128) float smem[];
+    __shared__ __align__(8) uint64_t mbar[2];
+
+    const int n = prog.n_dofs;
+    const bool has_qdr = args.qd_ref != nullptr, has_f = args.f != nullptr, has_lim = args.lim != nullptr;
+    const int n_in = 1 + (int)has_qdr + (int)has_f;
+    const PDRolloutSmem L(T, n, prog.n_links, prog.n_slots, n_in, args.per_row != 0);
+    float* s_tau = smem + L.tau;
+    float* s_qdd = smem + L.qdd;
+    float* s_kp = smem + L.kp;
+    float* s_kd = smem + L.kd;
+    float* s_lim = smem + L.lim;
+    float* s_tab = smem + L.table;
+    float* s_link = smem + L.link;
+    float* s_slot = smem + L.slots;
+    const int tid = threadIdx.x;
+    const int o_f = (has_qdr ? 2 : 1) * T * n;          // tiles of one input buffer: q_ref | qd_ref | f
+
+    const RolloutPipeline<T> pipe(mbar, smem + L.q, smem + L.qd, smem + L.in, args.q_ref, args.qd_ref, args.f, args.q, args.qd,
+                                  n, args.batch, args.n_steps, args.dt, args.aligned);
+    pipe.begin(args.q0, args.qd0);
+    if (args.per_row) {
+        coop_copy(s_kp, args.kp + pipe.tile_off, pipe.tile_floats, pipe.vec_ok);
+        coop_copy(s_kd, args.kd + pipe.tile_off, pipe.tile_floats, pipe.vec_ok);
+    } else {
+        coop_copy(s_kp, args.kp, n, false);
+        coop_copy(s_kd, args.kd, n, false);
+    }
+    if (has_lim) coop_copy(s_lim, args.lim, n, false);
+    if (fold.n_red > 0) stage_folded_table(s_tab, s_link, args.table, fold, prog, T);
+    else stage_canonical_table(s_tab, args.table, prog, T);
+    __syncthreads();
+
+    const int gain_row = args.per_row ? tid * n : 0;
+    for (int t = 0; t < args.n_steps; ++t) {
+        const float* s_it = pipe.fetch(t);
+        float* s_taut = s_tau + (t & 1) * T * n;
+        float* s_qddt = s_qdd + (t & 1) * T * n;
+        if (tid < pipe.valid) {
+            const float* qr = pipe.s_q + tid * n;
+            const float* qdr = pipe.s_qd + tid * n;
+            const float* ref = s_it + tid * n;
+            float* taur = s_taut + tid * n;
+            for (int k = 0; k < n; ++k) {
+                float e, ed;
+                const float u = pd_command(ref[k], qr[k], has_qdr ? ref[T * n + k] : 0.f, qdr[k], has_f ? ref[o_f + k] : 0.f,
+                                           s_kp[gain_row + k], s_kd[gain_row + k], e, ed);
+                taur[k] = has_lim ? pd_clamp(u, s_lim[k]) : u;
+            }
+            aba_body<T>(prog, s_tab, qr, qdr, taur, s_qddt + tid * n, s_link + tid, s_slot + tid, args.flags);
+        }
+        pipe.integrate_and_store(t, s_qddt + tid * n, 1, args.tau, s_taut, args.qdd, s_qddt);
+    }
+    pipe.finish();
+}
+
 // ---------------------------------------------------------------------------------------------
-// adjoint: the element-wise update between two ABA adjoint launches
+// adjoint: the element-wise update between two ABA adjoint launches, the post-update of step s = t + 1 fused with the
+// pre-update of step t.  Feedback adds the PD terms to the post-update; without it the fields of the feedback block are
+// unused.
 // ---------------------------------------------------------------------------------------------
 struct AdjStepArgs {
     float* a_q;                 // running adjoints of q_t / qd_t  [B, n]
     float* a_qd;
     float* g_step;              // g_qdd_t handed to the ABA adjoint
-    const float* gq;            // ABA adjoint of step t + 1 (post-update; unused when first)
+    const float* gq;            // ABA adjoint of step s (post-update; unused when first)
     const float* gqd;
+    // feedback: step s of the post-update -- its state, inputs, upstream g_tau (NULL = zero) and outputs (NULL = not wanted)
+    const float* gf;
+    const float* qs;
+    const float* qds;
+    const float* q_ref;
+    const float* qd_ref;
+    const float* f;
+    const float* g_tau;
+    float* f_grad;
+    float* q_ref_grad;
+    float* qd_ref_grad;
+    float* kp_grad;             // [B, n] running sums over the steps (NULL = not wanted)
+    float* kd_grad;
+    const float* kp;
+    const float* kd;
+    const float* lim;
+    int32_t n;
+    int32_t per_row;
+    int32_t last_post;          // s = T - 1: kp_grad / kd_grad are written rather than accumulated
+    // step t of the pre-update
     const float* g_q;           // upstream gradients of step t, NULL = zero
     const float* g_qd;
     const float* g_qdd;
@@ -182,12 +333,32 @@ struct AdjStepArgs {
     int32_t final;              // after step 0: post-update only, written to out_q / out_qd
 };
 
+template <bool Feedback>
 __global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStepArgs a) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.count; i += (int64_t)gridDim.x * blockDim.x) {
         float aq = 0.f, aqd = 0.f;
-        if (!a.first) {                                        // post-update of step t + 1
-            aq = __fadd_rn(a.a_q[i], a.gq[i]);
-            aqd = __fadd_rn(a.a_qd[i], a.gqd[i]);
+        if (!a.first) {                                        // post-update of step s
+            if constexpr (Feedback) {
+                const int k = (int)(i % a.n);
+                const int64_t gi = a.per_row ? i : k;
+                const float kp = a.kp[gi], kd = a.kd[gi];
+                float e, ed;
+                const float u = pd_command(a.q_ref[i], a.qs[i], a.qd_ref ? a.qd_ref[i] : 0.f, a.qds[i], a.f ? a.f[i] : 0.f, kp,
+                                           kd, e, ed);
+                float gu = a.gf[i];
+                if (a.g_tau != nullptr) gu = __fadd_rn(gu, a.g_tau[i]);
+                if (a.lim != nullptr && !(u >= -a.lim[k] && u <= a.lim[k])) gu = 0.f;   // torch.clamp's rule: equality passes
+                aq = __fsub_rn(__fadd_rn(a.a_q[i], a.gq[i]), __fmul_rn(kp, gu));
+                aqd = __fsub_rn(__fadd_rn(a.a_qd[i], a.gqd[i]), __fmul_rn(kd, gu));
+                if (a.f_grad != nullptr) a.f_grad[i] = gu;
+                if (a.q_ref_grad != nullptr) a.q_ref_grad[i] = __fmul_rn(kp, gu);
+                if (a.qd_ref_grad != nullptr) a.qd_ref_grad[i] = __fmul_rn(kd, gu);
+                if (a.kp_grad != nullptr) a.kp_grad[i] = a.last_post ? __fmul_rn(gu, e) : __fadd_rn(a.kp_grad[i], __fmul_rn(gu, e));
+                if (a.kd_grad != nullptr) a.kd_grad[i] = a.last_post ? __fmul_rn(gu, ed) : __fadd_rn(a.kd_grad[i], __fmul_rn(gu, ed));
+            } else {
+                aq = __fadd_rn(a.a_q[i], a.gq[i]);
+                aqd = __fadd_rn(a.a_qd[i], a.gqd[i]);
+            }
         }
         if (a.final) {
             if (a.out_q != nullptr) a.out_q[i] = aq;
@@ -208,14 +379,35 @@ __global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStep
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+// "rnea_fold", as drmb200_forward_dynamics, and the checks both forward rollouts start with
+static int rollout_program(const drmb200_topology_t* topo, int64_t batch, int32_t n_steps, FoldChoice* fc) {
+    const int rc = select_fold(topo, false, fc);
+    if (rc != DRMB200_OK) return rc;
+    if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
+    return DRMB200_OK;
+}
+
+// 64 configurations per CTA when that still gives every SM a CTA and the per-link state leaves room for two CTAs per SM;
+// 32 otherwise -- rollout batches are often below one wave of 64-thread CTAs, and a CTA stays resident for all steps.
+// floats_of(T) is the kernel's dynamic shared memory in floats.
+template <auto Kern64, auto Kern32, typename Args, typename F>
+static int launch_rollout(const FoldChoice& fc, int64_t batch, F floats_of, const char* what, const Args& args,
+                          cudaStream_t stream) {
+    const TileChoice c = tile_64_or_32([&](int T) { return (size_t)floats_of(T) * sizeof(float); }, 0,
+                                       (batch + 63) / 64 >= device_sm_count());
+    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
+    const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    return c.tile == 64 ? launch_kernel<Kern64>(tiles, 64, c.bytes, stream, false, what, *fc.prog, fc.fold, args)
+                        : launch_kernel<Kern32>(tiles, 32, c.bytes, stream, false, what, *fc.prog, fc.fold, args);
+}
+
 int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
                                     const float* f, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q,
                                     float* qd, float* qdd, cudaStream_t stream) {
     FoldChoice fc;
-    const int rc = select_fold(topo, false, &fc);                   // "rnea_fold", as drmb200_forward_dynamics
+    const int rc = rollout_program(topo, batch, n_steps, &fc);
     if (rc != DRMB200_OK) return rc;
     const TreeProgram& prog = *fc.prog;
-    if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
     if (batch == 0 || n_steps == 0 || prog.n_dofs == 0) return DRMB200_OK;
     if (table == nullptr || q0 == nullptr || qd0 == nullptr || f == nullptr || q == nullptr || qd == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
 
@@ -223,24 +415,116 @@ int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float*
     args.table = table; args.q0 = q0; args.qd0 = qd0; args.f = f; args.q = q; args.qd = qd; args.qdd = qdd;
     args.batch = batch; args.n_steps = n_steps; args.dt = dt; args.flags = flags;
     args.aligned = aligned16(q0, qd0, f, q, qd, qdd) && ((batch * prog.n_dofs) & 3) == 0;
-
-    // 64 configurations per CTA when that still gives every SM a CTA and the per-link state leaves room for two CTAs per
-    // SM; 32 otherwise -- rollout batches are often below one wave of 64-thread CTAs, and a CTA stays resident for all steps
-    const TileChoice c = tile_64_or_32([&](int T) {
-        return (size_t)RolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats * sizeof(float);
-    }, 0, (batch + 63) / 64 >= device_sm_count());
-    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
-    const int64_t tiles = (batch + c.tile - 1) / c.tile;
-    return c.tile == 64 ? launch_kernel<rollout_kernel<64>>(tiles, 64, c.bytes, stream, false, "rollout", prog, fc.fold, args)
-                        : launch_kernel<rollout_kernel<32>>(tiles, 32, c.bytes, stream, false, "rollout", prog, fc.fold, args);
+    return launch_rollout<rollout_kernel<64>, rollout_kernel<32>>(fc, batch, [&](int T) {
+        return RolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats;
+    }, "rollout", args, stream);
 }
 
-static int64_t round256(int64_t bytes) { return (bytes + 255) & ~(int64_t)255; }
+int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0, const float* q_ref,
+                      const float* qd_ref, const float* f, const float* kp, const float* kd, int32_t gains_per_row,
+                      const float* effort_limit, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q, float* qd,
+                      float* qdd, float* tau, cudaStream_t stream) {
+    FoldChoice fc;
+    const int rc = rollout_program(topo, batch, n_steps, &fc);
+    if (rc != DRMB200_OK) return rc;
+    const TreeProgram& prog = *fc.prog;
+    if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
+    if (batch == 0 || n_steps == 0 || prog.n_dofs == 0) return DRMB200_OK;
+    if (table == nullptr || q0 == nullptr || qd0 == nullptr || q_ref == nullptr || kp == nullptr || kd == nullptr ||
+        q == nullptr || qd == nullptr || tau == nullptr) {
+        set_error("null pointer argument");
+        return DRMB200_EINVAL;
+    }
 
-// [ABA adjoint workspace | a_q | a_qd | g_qdd_t | gq | gqd], each [B, n] fp32
-int64_t forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
+    PDRolloutArgs args;
+    args.table = table; args.q0 = q0; args.qd0 = qd0; args.q_ref = q_ref; args.qd_ref = qd_ref; args.f = f;
+    args.kp = kp; args.kd = kd; args.lim = effort_limit; args.q = q; args.qd = qd; args.qdd = qdd; args.tau = tau;
+    args.batch = batch; args.n_steps = n_steps; args.dt = dt; args.flags = flags; args.per_row = gains_per_row;
+    args.aligned = aligned16(q0, qd0, q_ref, qd_ref, f, q, qd, qdd, tau) && (!gains_per_row || aligned16(kp, kd)) &&
+                   ((batch * prog.n_dofs) & 3) == 0;
+    const int n_in = 1 + (qd_ref != nullptr) + (f != nullptr);
+    return launch_rollout<pd_rollout_kernel<64>, pd_rollout_kernel<32>>(fc, batch, [&](int T) {
+        return PDRolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots, n_in, gains_per_row != 0).total_floats;
+    }, "pd rollout", args, stream);
+}
+
+// The reverse-time adjoint of both rollouts.  Workspace: [ABA adjoint workspace | a_q | a_qd | g_qdd_t | gq | gqd (| gf
+// with feedback)], each [B, n] fp32.
+int64_t rollout_adjoint_workspace_bytes(const drmb200_topology_t* topo, int64_t batch, bool feedback) {
     if (topo == nullptr || topo->n_links < 1 || topo->n_links > DRMB200_MAX_LINKS || batch < 0) return 0;
-    return round256(forward_dynamics_backward_workspace_bytes(topo, batch)) + 5 * round256(batch * topo->n_dofs * (int64_t)sizeof(float));
+    return round256(forward_dynamics_backward_workspace_bytes(topo, batch)) +
+           (feedback ? 6 : 5) * round256(batch * topo->n_dofs * (int64_t)sizeof(float));
+}
+
+// tau: the [T, B, n] torques the forward applied.  Open loop (fb == NULL): f_grad receives the ABA adjoint's f gradient.
+// With feedback, fb holds the kernel's PD fields and [T, B, n] bases of its per-step inputs and gradients, which the loop
+// offsets to each step; the ABA adjoint's f gradient goes to the gf slice.  want_final: q0_grad, qd0_grad or a feedback
+// gradient is wanted, so the post-update of step 0 runs.
+static int rollout_adjoint(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
+                           const float* tau, int64_t batch, int32_t n_steps, float dt, uint32_t flags, const float* q,
+                           const float* qd, const float* g_q, const float* g_qd, const float* g_qdd, float* q0_grad,
+                           float* qd0_grad, float* f_grad, float* table_grad, const AdjStepArgs* fb, bool want_final,
+                           void* workspace, cudaStream_t stream) {
+    const int64_t count = batch * topo->n_dofs;
+    const int64_t slice = round256(count * (int64_t)sizeof(float));
+    char* ws = static_cast<char*>(workspace);
+    void* fd_ws = ws;
+    ws += round256(forward_dynamics_backward_workspace_bytes(topo, batch));
+    float* a_q = reinterpret_cast<float*>(ws);
+    float* a_qd = reinterpret_cast<float*>(ws + slice);
+    float* g_step = reinterpret_cast<float*>(ws + 2 * slice);
+    float* gq = reinterpret_cast<float*>(ws + 3 * slice);
+    float* gqd = reinterpret_cast<float*>(ws + 4 * slice);
+    float* gf = fb ? reinterpret_cast<float*>(ws + 5 * slice) : nullptr;
+
+    int64_t blocks = (count + 255) / 256;
+    if (blocks > (int64_t)device_sm_count() * 8) blocks = (int64_t)device_sm_count() * 8;
+    auto step_kernel = [&](const AdjStepArgs& a) {
+        return fb ? launch_kernel<rollout_adjoint_step_kernel<true>>(blocks, 256, 0, stream, false, "pd rollout adjoint step", a)
+                  : launch_kernel<rollout_adjoint_step_kernel<false>>(blocks, 256, 0, stream, false, "rollout adjoint step", a);
+    };
+    auto at = [&](auto* p, int s) { return p ? p + (int64_t)s * count : nullptr; };
+
+    AdjStepArgs a = fb ? *fb : AdjStepArgs{};
+    a.a_q = a_q; a.a_qd = a_qd; a.g_step = g_step; a.gq = gq; a.gqd = gqd; a.gf = gf;
+    a.n = topo->n_dofs; a.count = count; a.dt = dt;
+    // the feedback post-update of step s reads its state (q0 / qd0, then the forward's outputs) and inputs, writes its
+    // gradients
+    auto post = [&](int s) {
+        if (fb == nullptr) return;
+        a.qs = s == 0 ? q0 : q + (int64_t)(s - 1) * count;
+        a.qds = s == 0 ? qd0 : qd + (int64_t)(s - 1) * count;
+        a.q_ref = at(fb->q_ref, s); a.qd_ref = at(fb->qd_ref, s); a.f = at(fb->f, s); a.g_tau = at(fb->g_tau, s);
+        a.f_grad = at(fb->f_grad, s); a.q_ref_grad = at(fb->q_ref_grad, s); a.qd_ref_grad = at(fb->qd_ref_grad, s);
+        a.last_post = s == n_steps - 1;
+    };
+    for (int t = n_steps - 1; t >= 0; --t) {
+        a.first = (t == n_steps - 1) ? 1 : 0;
+        a.final = 0;
+        if (!a.first) post(t + 1);
+        a.g_q = at(g_q, t);
+        a.g_qd = at(g_qd, t);
+        a.g_qdd = at(g_qdd, t);
+        int rc = step_kernel(a);
+        if (rc != DRMB200_OK) return rc;
+        const float* qt = t == 0 ? q0 : q + (int64_t)(t - 1) * count;     // step inputs: (q0, qd0), then the forward's outputs
+        const float* qdt = t == 0 ? qd0 : qd + (int64_t)(t - 1) * count;
+        rc = forward_dynamics_backward_device(topo, table, qt, qdt, tau + (int64_t)t * count, batch, flags, g_step, gq, gqd,
+                                              fb ? gf : at(f_grad, t), table_grad, fd_ws, stream,
+                                              /*accumulate_partials=*/t != n_steps - 1, /*reduce=*/t == 0);
+        if (rc != DRMB200_OK) return rc;
+    }
+    if (!want_final) return DRMB200_OK;
+    a.first = 0;
+    a.final = 1;
+    post(0);
+    a.out_q = q0_grad;
+    a.out_qd = qd0_grad;
+    return step_kernel(a);
+}
+
+int64_t forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
+    return rollout_adjoint_workspace_bytes(topo, batch, false);
 }
 
 int forward_dynamics_rollout_backward_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
@@ -257,48 +541,40 @@ int forward_dynamics_rollout_backward_device(const drmb200_topology_t* topo, con
         return DRMB200_EINVAL;
     }
     if (workspace == nullptr) { set_error("rollout backward needs its workspace (drmb200_forward_dynamics_rollout_backward_workspace_bytes)"); return DRMB200_EINVAL; }
+    return rollout_adjoint(topo, table, q0, qd0, f, batch, n_steps, dt, flags, q, qd, g_q, g_qd, g_qdd, q0_grad, qd0_grad,
+                           f_grad, table_grad, nullptr, q0_grad != nullptr || qd0_grad != nullptr, workspace, stream);
+}
 
-    const int64_t count = batch * topo->n_dofs;
-    const int64_t slice = round256(count * (int64_t)sizeof(float));
-    char* ws = static_cast<char*>(workspace);
-    void* fd_ws = ws;
-    ws += round256(forward_dynamics_backward_workspace_bytes(topo, batch));
-    float* a_q = reinterpret_cast<float*>(ws);
-    float* a_qd = reinterpret_cast<float*>(ws + slice);
-    float* g_step = reinterpret_cast<float*>(ws + 2 * slice);
-    float* gq = reinterpret_cast<float*>(ws + 3 * slice);
-    float* gqd = reinterpret_cast<float*>(ws + 4 * slice);
+int64_t pd_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
+    return rollout_adjoint_workspace_bytes(topo, batch, true);
+}
 
-    int64_t blocks = (count + 255) / 256;
-    if (blocks > (int64_t)device_sm_count() * 8) blocks = (int64_t)device_sm_count() * 8;
-    auto step_kernel = [&](const AdjStepArgs& a) {
-        return launch_kernel<rollout_adjoint_step_kernel>(blocks, 256, 0, stream, false, "rollout adjoint step", a);
-    };
-
-    AdjStepArgs a = {};
-    a.a_q = a_q; a.a_qd = a_qd; a.g_step = g_step; a.gq = gq; a.gqd = gqd; a.count = count; a.dt = dt;
-    for (int t = n_steps - 1; t >= 0; --t) {
-        const int64_t off = (int64_t)t * count;
-        a.first = (t == n_steps - 1) ? 1 : 0;
-        a.final = 0;
-        a.g_q = g_q ? g_q + off : nullptr;
-        a.g_qd = g_qd ? g_qd + off : nullptr;
-        a.g_qdd = g_qdd ? g_qdd + off : nullptr;
-        int rc = step_kernel(a);
-        if (rc != DRMB200_OK) return rc;
-        const float* qt = t == 0 ? q0 : q + off - count;        // step inputs: (q0, qd0), then the forward's outputs
-        const float* qdt = t == 0 ? qd0 : qd + off - count;
-        rc = forward_dynamics_backward_device(topo, table, qt, qdt, f + off, batch, flags, g_step, gq, gqd,
-                                              f_grad ? f_grad + off : nullptr, table_grad, fd_ws, stream,
-                                              /*accumulate_partials=*/t != n_steps - 1, /*reduce=*/t == 0);
-        if (rc != DRMB200_OK) return rc;
+int pd_rollout_backward_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,
+                               const float* q_ref, const float* qd_ref, const float* f, const float* kp, const float* kd,
+                               int32_t gains_per_row, const float* effort_limit, int64_t batch, int32_t n_steps, float dt,
+                               uint32_t flags, const float* q, const float* qd, const float* tau, const float* g_q,
+                               const float* g_qd, const float* g_qdd, const float* g_tau, float* q0_grad, float* qd0_grad,
+                               float* q_ref_grad, float* qd_ref_grad, float* f_grad, float* kp_grad, float* kd_grad,
+                               float* table_grad, void* workspace, cudaStream_t stream) {
+    if (topo == nullptr) { set_error("null topology"); return DRMB200_EINVAL; }
+    if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
+    if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
+    if (batch == 0 || n_steps == 0 || topo->n_dofs == 0) return DRMB200_OK;
+    const bool want_elementwise = q0_grad || qd0_grad || q_ref_grad || qd_ref_grad || f_grad || kp_grad || kd_grad;
+    if (!want_elementwise && table_grad == nullptr) return DRMB200_OK;
+    if (table == nullptr || q0 == nullptr || qd0 == nullptr || q_ref == nullptr || kp == nullptr || kd == nullptr ||
+        tau == nullptr || (n_steps > 1 && (q == nullptr || qd == nullptr))) {
+        set_error("null pointer argument");
+        return DRMB200_EINVAL;
     }
-    if (q0_grad == nullptr && qd0_grad == nullptr) return DRMB200_OK;
-    a.first = 0;
-    a.final = 1;
-    a.out_q = q0_grad;
-    a.out_qd = qd0_grad;
-    return step_kernel(a);
+    if (workspace == nullptr) { set_error("pd rollout backward needs its workspace (drmb200_pd_rollout_backward_workspace_bytes)"); return DRMB200_EINVAL; }
+
+    AdjStepArgs fb = {};
+    fb.q_ref = q_ref; fb.qd_ref = qd_ref; fb.f = f; fb.g_tau = g_tau;
+    fb.f_grad = f_grad; fb.q_ref_grad = q_ref_grad; fb.qd_ref_grad = qd_ref_grad;
+    fb.kp_grad = kp_grad; fb.kd_grad = kd_grad; fb.kp = kp; fb.kd = kd; fb.lim = effort_limit; fb.per_row = gains_per_row;
+    return rollout_adjoint(topo, table, q0, qd0, tau, batch, n_steps, dt, flags, q, qd, g_q, g_qd, g_qdd, q0_grad, qd0_grad,
+                           nullptr, table_grad, &fb, want_elementwise, workspace, stream);
 }
 
 }  // namespace drm

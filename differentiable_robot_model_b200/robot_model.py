@@ -871,6 +871,29 @@ class DifferentiableRobotModel(torch.nn.Module):
             self._limit_cache = (lower, upper)
         return self._limit_cache
 
+    def _check_rollout_inputs(self, required, optional, steps):
+        """The argument checks every rollout starts with: each ``(name, tensor)`` of ``required``, and of ``optional``
+        unless None, is a float32 tensor on the module's device; ``q0`` / ``qd0`` (the first two) are one [batch_size x
+        n_dofs] or [n_dofs] shape; the input named ``steps`` is [T x batch_size x n_dofs] (or [T x n_dofs]).  Returns
+        whether the inputs are 1-D (one row without a batch dimension)."""
+        for name, t in tuple(required) + tuple((name, t) for name, t in optional if t is not None):
+            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
+            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
+            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
+        q0, qd0, seq = required[0][1], required[1][1], dict(required)[steps]
+        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
+        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
+        assert q0.shape[-1] == self._n_dofs, f"expected {self._n_dofs} joints, got {q0.shape[-1]}"
+        assert seq.ndim == q0.ndim + 1 and seq.shape[1:] == q0.shape, \
+            f"{steps} must be [T x batch_size x n_dofs] (or [T x n_dofs])."
+        return q0.ndim == 1
+
+    @staticmethod
+    def _rollout_batch_dim(q0, qd0, *per_step):
+        """1-D rollout inputs with the batch dimension of one row added: ``q0`` / ``qd0`` in front, every per-step (or
+        per-link) tensor after its leading dimension; None stays None."""
+        return (q0.unsqueeze(0), qd0.unsqueeze(0)) + tuple(None if t is None else t.unsqueeze(1) for t in per_step)
+
     def compute_forward_dynamics_rollout(
         self,
         q0: torch.Tensor,
@@ -896,17 +919,9 @@ class DifferentiableRobotModel(torch.nn.Module):
         Returns: time-major ``(q, qd, qdd)``, each [T x batch_size x n_dofs] (or [T x n_dofs]), with ``q[t] = q_{t+1}``,
         ``qd[t] = qd_{t+1}`` and ``qdd[t] = qdd_t``.  Differentiable w.r.t. q0, qd0, f and every learnable link parameter
         (the articulated-body adjoint stepped backwards in time).  Argument errors raise ``AssertionError``."""
-        for name, t in (("q0", q0), ("qd0", qd0), ("f", f)):
-            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
-            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
-            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
-        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
-        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
-        assert q0.shape[-1] == self._n_dofs, f"expected {self._n_dofs} joints, got {q0.shape[-1]}"
-        assert f.ndim == q0.ndim + 1 and f.shape[1:] == q0.shape, "f must be [T x batch_size x n_dofs] (or [T x n_dofs])."
-        squeeze = q0.ndim == 1
+        squeeze = self._check_rollout_inputs((("q0", q0), ("qd0", qd0), ("f", f)), (), "f")
         if squeeze:
-            q0, qd0, f = q0.unsqueeze(0), qd0.unsqueeze(0), f.unsqueeze(1)
+            q0, qd0, f = self._rollout_batch_dim(q0, qd0, f)
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
         table = self._link_table()
         dt = float(dt)
@@ -969,27 +984,16 @@ class DifferentiableRobotModel(torch.nn.Module):
         included) but are not differentiable.  Argument errors raise ``AssertionError``."""
         links = self._contact_links(link_names)
         E = len(links)
-        for name, t in (("q0", q0), ("qd0", qd0), ("f", f), ("target_pos", target_pos), ("target_quat", target_quat)):
-            if t is None and name.startswith("target"):
-                continue
-            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
-            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
-            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
-        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
-        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
-        assert q0.shape[-1] == self._n_dofs, f"expected {self._n_dofs} joints, got {q0.shape[-1]}"
-        assert f.ndim == q0.ndim + 1 and f.shape[1:] == q0.shape, "f must be [T x batch_size x n_dofs] (or [T x n_dofs])."
+        squeeze = self._check_rollout_inputs((("q0", q0), ("qd0", qd0), ("f", f)),
+                                             (("target_pos", target_pos), ("target_quat", target_quat)), "f")
         if position_only:
             assert target_quat is None, "target_quat must be None with position_only"
         else:
             assert (target_pos is None) == (target_quat is None), "give target_pos and target_quat together in pose mode"
         stabilization = float(stabilization)
         assert stabilization >= 0 and stabilization != float("inf"), "stabilization must be finite and >= 0"
-        squeeze = q0.ndim == 1
         if squeeze:
-            q0, qd0, f = q0.unsqueeze(0), qd0.unsqueeze(0), f.unsqueeze(1)
-            target_pos = None if target_pos is None else target_pos.unsqueeze(1)
-            target_quat = None if target_quat is None else target_quat.unsqueeze(1)
+            q0, qd0, f, target_pos, target_quat = self._rollout_batch_dim(q0, qd0, f, target_pos, target_quat)
         B = q0.shape[0]
         assert target_pos is None or tuple(target_pos.shape) == (E, B, 3), "target_pos must be [n_links x batch_size x 3]"
         assert target_quat is None or tuple(target_quat.shape) == (E, B, 4), "target_quat must be [n_links x batch_size x 4]"
@@ -1018,7 +1022,7 @@ class DifferentiableRobotModel(torch.nn.Module):
     ) -> ControlledRollout:
         r"""Simulate a joint-space PD controller tracking reference trajectories: :meth:`compute_forward_dynamics_rollout`
         with the torque of every step computed from the current state, all ``T`` steps in ONE launch
-        (``csrc/pd_rollout.cu``).  From ``(q_0, qd_0) = (q0, qd0)``, step ``t`` computes in fp32, in this order::
+        (``csrc/rollout.cu``).  From ``(q_0, qd_0) = (q0, qd0)``, step ``t`` computes in fp32, in this order::
 
             u = f[t] + kp * (q_ref[t] - q) + kd * (qd_ref[t] - qd)      # qd_ref / f None: zero tensors
             u = torch.clamp(u, -effort_limit, effort_limit)             # only when effort_limit is given
@@ -1043,20 +1047,9 @@ class DifferentiableRobotModel(torch.nn.Module):
         Differentiable w.r.t. q0, qd0, q_ref, qd_ref, f, kp, kd and every learnable link parameter (the articulated-body
         adjoint stepped backwards in time, the clamp passing gradients where ``-effort_limit <= u <= effort_limit``); not
         w.r.t. dt or effort_limit.  Argument errors raise ``AssertionError``."""
-        named = (("q0", q0), ("qd0", qd0), ("q_ref", q_ref), ("kp", kp), ("kd", kd), ("qd_ref", qd_ref), ("f", f),
-                 ("effort_limit", effort_limit))
-        for name, t in named:
-            if t is None and name in ("qd_ref", "f", "effort_limit"):
-                continue
-            assert type(t) is torch.Tensor, f"{name} must be a torch.Tensor"
-            assert t.device.type == self._device.type, f"Input argument of different device as module: {name}"
-            assert t.dtype == torch.float32, f"{name} must be float32 (got {t.dtype})"
+        squeeze = self._check_rollout_inputs((("q0", q0), ("qd0", qd0), ("q_ref", q_ref), ("kp", kp), ("kd", kd)),
+                                             (("qd_ref", qd_ref), ("f", f), ("effort_limit", effort_limit)), "q_ref")
         n = self._n_dofs
-        assert q0.ndim in (1, 2), "q0 must have ndim of 1 or 2."
-        assert qd0.shape == q0.shape, "q0 and qd0 must have the same shape."
-        assert q0.shape[-1] == n, f"expected {n} joints, got {q0.shape[-1]}"
-        assert q_ref.ndim == q0.ndim + 1 and q_ref.shape[1:] == q0.shape, \
-            "q_ref must be [T x batch_size x n_dofs] (or [T x n_dofs])."
         for name, t in (("qd_ref", qd_ref), ("f", f)):
             assert t is None or t.shape == q_ref.shape, f"{name} must have the shape of q_ref."
         gain_shapes = ((n,),) if q0.ndim == 1 else ((n,), tuple(q0.shape))
@@ -1071,11 +1064,8 @@ class DifferentiableRobotModel(torch.nn.Module):
                     and not torch.cuda.is_current_stream_capturing():
                 assert bool((effort_limit > 0).all()), "effort_limit must be > 0 (inf allowed) and not NaN."
                 self._checked_effort_limit = (weakref.ref(effort_limit), effort_limit._version)
-        squeeze = q0.ndim == 1
         if squeeze:
-            q0, qd0, q_ref = q0.unsqueeze(0), qd0.unsqueeze(0), q_ref.unsqueeze(1)
-            qd_ref = None if qd_ref is None else qd_ref.unsqueeze(1)
-            f = None if f is None else f.unsqueeze(1)
+            q0, qd0, q_ref, qd_ref, f = self._rollout_batch_dim(q0, qd0, q_ref, qd_ref, f)
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
         table = self._link_table()
         dt = float(dt)

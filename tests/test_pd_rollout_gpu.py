@@ -1,4 +1,4 @@
-"""GPU: PD-controlled rollouts (csrc/pd_rollout.cu) -- a diagonal joint-space PD law around T semi-implicit Euler steps of
+"""GPU: PD-controlled rollouts (csrc/rollout.cu) -- a diagonal joint-space PD law around T semi-implicit Euler steps of
 the articulated-body kernel in one launch, and its adjoint stepped backwards in time:
 
   * zero gains without a limit reproduce the open-loop rollout bit for bit;
