@@ -389,14 +389,31 @@ static int rollout_program(const drmb200_topology_t* topo, int64_t batch, int32_
 
 // 64 configurations per CTA when that still gives every SM a CTA and the per-link state leaves room for two CTAs per SM;
 // 32 otherwise -- rollout batches are often below one wave of 64-thread CTAs, and a CTA stays resident for all steps.
+// With Kern16 (the PD rollout's), a 32-row CTA that exceeds SMEM_CTA_MAX with the kernel's static shared memory falls
+// back to 16 rows, refused only when that still does not fit: the PD layout's input streams and per-row gains push a
+// 63-DoF chain past the limit at 32 rows.  The open-loop rollout's 32-row CTA fits every model the engine accepts.  A
+// folded model only needs the 16-row rung with more than 50 reduced links, whose per-link state (14 x 16 floats each)
+// still holds the fold's staging scratch (40 floats per original link, at most 64 links).
 // floats_of(T) is the kernel's dynamic shared memory in floats.
-template <auto Kern64, auto Kern32, typename Args, typename F>
+template <auto Kern64, auto Kern32, auto Kern16 = nullptr, typename Args, typename F>
 static int launch_rollout(const FoldChoice& fc, int64_t batch, F floats_of, const char* what, const Args& args,
                           cudaStream_t stream) {
-    const TileChoice c = tile_64_or_32([&](int T) { return (size_t)floats_of(T) * sizeof(float); }, 0,
-                                       (batch + 63) / 64 >= device_sm_count());
-    if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
+    auto bytes_of = [&](int T) { return (size_t)floats_of(T) * sizeof(float); };
+    TileChoice c = tile_64_or_32(bytes_of, 0, (batch + 63) / 64 >= device_sm_count());
+    size_t static_bytes = 0;
+    if constexpr (!std::is_same_v<decltype(Kern16), std::nullptr_t>) {
+        const int rc = static_smem_bytes<Kern32>(&static_bytes);
+        if (rc != DRMB200_OK) return rc;
+        if (c.bytes + static_bytes > SMEM_CTA_MAX) c = {16, bytes_of(16)};
+    }
+    if (c.bytes + static_bytes > SMEM_CTA_MAX) {
+        set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes + static_bytes);
+        return DRMB200_ELIMIT;
+    }
     const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    if constexpr (!std::is_same_v<decltype(Kern16), std::nullptr_t>) {
+        if (c.tile == 16) return launch_kernel<Kern16>(tiles, 16, c.bytes, stream, false, what, *fc.prog, fc.fold, args);
+    }
     return c.tile == 64 ? launch_kernel<Kern64>(tiles, 64, c.bytes, stream, false, what, *fc.prog, fc.fold, args)
                         : launch_kernel<Kern32>(tiles, 32, c.bytes, stream, false, what, *fc.prog, fc.fold, args);
 }
@@ -443,7 +460,7 @@ int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const 
     args.aligned = aligned16(q0, qd0, q_ref, qd_ref, f, q, qd, qdd, tau) && (!gains_per_row || aligned16(kp, kd)) &&
                    ((batch * prog.n_dofs) & 3) == 0;
     const int n_in = 1 + (qd_ref != nullptr) + (f != nullptr);
-    return launch_rollout<pd_rollout_kernel<64>, pd_rollout_kernel<32>>(fc, batch, [&](int T) {
+    return launch_rollout<pd_rollout_kernel<64>, pd_rollout_kernel<32>, pd_rollout_kernel<16>>(fc, batch, [&](int T) {
         return PDRolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots, n_in, gains_per_row != 0).total_floats;
     }, "pd rollout", args, stream);
 }

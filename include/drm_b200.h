@@ -315,8 +315,9 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
  *   q, qd, qdd, tau                [n_steps, B, n_dofs]   q[t] = q_{t+1}, qd[t] = qd_{t+1}, qdd[t] = qdd_t, tau[t] = tau_t;
  *                                  qdd may be NULL
  * No allocation, no synchronisation, graph-capturable.  Outputs must not alias inputs.  batch == 0 or n_steps == 0 is a
- * no-op.  DRMB200_EINVAL for a NULL required pointer or a negative size; DRMB200_ELIMIT when a 32-configuration CTA needs
- * more than 227 KB of shared memory (the message names the bytes).
+ * no-op.  DRMB200_EINVAL for a NULL required pointer or a negative size.  A CTA holds 64 or 32 configurations, or 16 when
+ * 32 need more than 227 KB of shared memory (per-row gains and all three input streams take a 63-DoF chain there);
+ * DRMB200_ELIMIT only when a 16-configuration CTA still needs more (the message names the bytes).
  */
 int drmb200_pd_rollout(const drmb200_topology_t* topo, const float* table,
                        const float* q0, const float* qd0, const float* q_ref, const float* qd_ref, const float* f,
