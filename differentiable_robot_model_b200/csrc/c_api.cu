@@ -126,6 +126,14 @@ int contact_dynamics_device(const drmb200_topology_t*, int32_t, const int32_t*, 
                             const float*, const float*, int64_t, uint32_t, int32_t, float, float*, float*, uint8_t*, cudaStream_t);
 int contact_impulse_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
                            const float*, int64_t, int32_t, float, float*, float*, uint8_t*, cudaStream_t);
+int64_t contact_backward_workspace_bytes(const drmb200_topology_t*, int32_t, const int32_t*, int32_t, int64_t);
+int contact_dynamics_backward_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                                     const float*, const float*, const float*, const float*, const uint8_t*, int64_t, uint32_t,
+                                     int32_t, float, const float*, const float*, float*, float*, float*, float*, float*, void*,
+                                     cudaStream_t);
+int contact_impulse_backward_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
+                                    const float*, const float*, const float*, const uint8_t*, int64_t, int32_t, float,
+                                    const float*, const float*, float*, float*, float*, float*, void*, cudaStream_t);
 int contact_rollout_device(const drmb200_topology_t*, int32_t, const int32_t*, const float*, const float*, const float*,
                            const float*, const float*, const float*, int64_t, int32_t, float, uint32_t, int32_t, float, float,
                            float*, float*, float*, float*, float*, uint8_t*, cudaStream_t);
@@ -503,6 +511,33 @@ int drmb200_contact_impulse(const drmb200_topology_t* topo, int32_t n_ee, const 
                             float regularization, float* qd_plus, float* impulse, uint8_t* solved, void* cuda_stream) {
     return drm::contact_impulse_device(topo, n_ee, ee_links, table, q, qd, velocity_ref, batch, position_only, regularization,
                                        qd_plus, impulse, solved, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int64_t drmb200_contact_backward_workspace_bytes(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links,
+                                                 int32_t position_only, int64_t batch) {
+    return drm::contact_backward_workspace_bytes(topo, n_ee, ee_links, position_only, batch);
+}
+
+int drmb200_contact_dynamics_backward(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                      const float* q, const float* qd, const float* f, const float* accel_ref, const float* qdd,
+                                      const float* force, const uint8_t* solved, int64_t batch, uint32_t flags,
+                                      int32_t position_only, float regularization, const float* g_qdd, const float* g_force,
+                                      float* q_grad, float* qd_grad, float* f_grad, float* accel_ref_grad, float* table_grad,
+                                      void* workspace, void* cuda_stream) {
+    return drm::contact_dynamics_backward_device(topo, n_ee, ee_links, table, q, qd, f, accel_ref, qdd, force, solved, batch,
+                                                 flags, position_only, regularization, g_qdd, g_force, q_grad, qd_grad, f_grad,
+                                                 accel_ref_grad, table_grad, workspace, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_contact_impulse_backward(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                     const float* q, const float* qd, const float* velocity_ref, const float* qd_plus,
+                                     const float* impulse, const uint8_t* solved, int64_t batch, int32_t position_only,
+                                     float regularization, const float* g_qd_plus, const float* g_impulse, float* q_grad,
+                                     float* qd_grad, float* velocity_ref_grad, float* table_grad, void* workspace,
+                                     void* cuda_stream) {
+    return drm::contact_impulse_backward_device(topo, n_ee, ee_links, table, q, qd, velocity_ref, qd_plus, impulse, solved,
+                                                batch, position_only, regularization, g_qd_plus, g_impulse, q_grad, qd_grad,
+                                                velocity_ref_grad, table_grad, workspace, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_contact_rollout(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,

@@ -57,6 +57,71 @@ __device__ __forceinline__ bool contact_solve(float* A, float* b, float* s, int 
     return true;
 }
 
+// The factorisation of contact_solve, kept for a solve with the transpose (contact_backward.cu): the same float operations
+// on A in the same order, so the pivot sequence and the solved decision are contact_solve's bit for bit.  On return
+// (true) s holds the scales, A the LU factors of P S A S (U on and above the diagonal, the multipliers of the unit lower L
+// below it, rows swapped in full) and piv[k T] the row swapped with row k at step k, as a float.
+template <int T>
+__device__ __forceinline__ bool contact_factor(float* A, float* s, float* piv, int M) {
+    const int rs = M * T;
+    for (int k = 0; k < M; ++k) {
+        const float d = fabsf(A[k * rs + k * T]);
+        if (!(d > 0.f) || !isfinite(d)) return false;
+        s[k * T] = 1.0f / sqrtf(d);
+    }
+    for (int i = 0; i < M; ++i) {
+        const float si = s[i * T];
+        for (int j = 0; j < M; ++j) A[i * rs + j * T] = si * A[i * rs + j * T] * s[j * T];
+    }
+    for (int k = 0; k < M; ++k) {
+        int p = k;
+        float best = fabsf(A[k * rs + k * T]);
+        for (int i = k + 1; i < M; ++i) {               // strictly larger: ties go to the lower row
+            const float v = fabsf(A[i * rs + k * T]);
+            if (v > best) { best = v; p = i; }
+        }
+        const float pv = A[p * rs + k * T];
+        if (!(fabsf(pv) > CONTACT_PIVOT_MIN) || !isfinite(pv)) return false;
+        piv[k * T] = (float)p;
+        if (p != k) {
+            for (int j = 0; j < M; ++j) {               // the multipliers (j < k) move with their rows
+                const float t = A[k * rs + j * T]; A[k * rs + j * T] = A[p * rs + j * T]; A[p * rs + j * T] = t;
+            }
+        }
+        const float inv = 1.0f / pv;
+        for (int i = k + 1; i < M; ++i) {
+            const float l = A[i * rs + k * T] * inv;
+            for (int j = k + 1; j < M; ++j) A[i * rs + j * T] = fmaf(-l, A[k * rs + j * T], A[i * rs + j * T]);
+            A[i * rs + k * T] = l;
+        }
+    }
+    return true;
+}
+
+// Solves A^T x = b (b overwritten with x) on the factors contact_factor left: with A~ = S A S and P A~ = L U,
+// A~^T y = S b is U^T L^T P y = S b (forward substitution with U^T, back substitution with the unit L^T, then the swaps in
+// reverse order), and x = S y.
+template <int T>
+__device__ __forceinline__ void contact_solve_transposed(const float* A, float* b, const float* s, const float* piv, int M) {
+    const int rs = M * T;
+    for (int i = 0; i < M; ++i) b[i * T] *= s[i * T];
+    for (int i = 0; i < M; ++i) {                       // U^T z = S b
+        float x = b[i * T];
+        for (int j = 0; j < i; ++j) x = fmaf(-A[j * rs + i * T], b[j * T], x);
+        b[i * T] = x / A[i * rs + i * T];
+    }
+    for (int i = M - 1; i >= 0; --i) {                  // L^T w = z
+        float x = b[i * T];
+        for (int j = i + 1; j < M; ++j) x = fmaf(-A[j * rs + i * T], b[j * T], x);
+        b[i * T] = x;
+    }
+    for (int k = M - 1; k >= 0; --k) {                  // y = P^T w
+        const int p = (int)piv[k * T];
+        if (p != k) { const float t = b[k * T]; b[k * T] = b[p * T]; b[p * T] = t; }
+    }
+    for (int i = 0; i < M; ++i) b[i * T] *= s[i * T];
+}
+
 // One row of the contact dynamics (IMPULSE: the contact impulse), thread tid of a CTA of T rows:
 //   1. osd_walk: J, J qd and Jdot qd (and, with POSES, every link's pose);   then the statements AFTER_WALK, which may
 //      write the row's reference slots;

@@ -148,9 +148,14 @@ __device__ __forceinline__ void aba_unit_response(const TreeProgram& prog, const
 // the row used as the right-hand side and the response of each sweep (both overwritten).  The product is formed in the
 // smaller space:  M <= n_u: M sweeps with tau = J^T e_k give the columns of G J^T;  M > n_u: n_u sweeps with tau = e_j,
 // then inv += (J G e_j) J[:, j]^T.
-template <int T>
+//
+// GDOT (contact_backward.cu): also sdot [M] (slot-major) = J G^T g for the row's n floats g, from the same sweeps -- entry k
+// is g . (G J^T e_k) when M <= n_u; when M > n_u each sweep gives (G^T g)_j = g . (G e_j) and sdot += J[:, j] (G^T g)_j.
+// The false instantiation is the code without these dot products.
+template <int T, bool GDOT = false>
 __device__ __forceinline__ void osd_inverse_inertia(const TreeProgram& prog, const UnionProgram& P, const float* s_tab, int M,
-                                                    const float* J, float* inv, float* frow, float* xrow, float* lk0, float* sl0) {
+                                                    const float* J, float* inv, float* frow, float* xrow, float* lk0, float* sl0,
+                                                    const float* g = nullptr, float* sdot = nullptr) {
     const int n = prog.n_dofs;
     const int n_u = P.n_u;
     const int rs = n_u * T;
@@ -164,9 +169,15 @@ __device__ __forceinline__ void osd_inverse_inertia(const TreeProgram& prog, con
                 for (int u = 0; u < n_u; ++u) s = fmaf(J[m * rs + u * T], xrow[P.u_dof[u]], s);
                 inv[(m * M + k) * T] = s;
             }
+            if constexpr (GDOT) {
+                float s = 0.f;
+                for (int c = 0; c < n; ++c) s = fmaf(g[c], xrow[c], s);
+                sdot[k * T] = s;
+            }
         }
     } else {
         for (int i = 0; i < M * M; ++i) inv[i * T] = 0.f;
+        if constexpr (GDOT) for (int m = 0; m < M; ++m) sdot[m * T] = 0.f;
         for (int j = 0; j < n_u; ++j) {     // += (J G e_j) J[:, j]^T
             for (int c = 0; c < n; ++c) frow[c] = 0.f;
             frow[P.u_dof[j]] = 1.f;
@@ -175,6 +186,11 @@ __device__ __forceinline__ void osd_inverse_inertia(const TreeProgram& prog, con
                 float y = 0.f;
                 for (int u = 0; u < n_u; ++u) y = fmaf(J[m * rs + u * T], xrow[P.u_dof[u]], y);
                 for (int k = 0; k < M; ++k) inv[(m * M + k) * T] = fmaf(y, J[k * rs + j * T], inv[(m * M + k) * T]);
+            }
+            if constexpr (GDOT) {
+                float t = 0.f;
+                for (int c = 0; c < n; ++c) t = fmaf(g[c], xrow[c], t);
+                for (int m = 0; m < M; ++m) sdot[m * T] = fmaf(J[m * rs + j * T], t, sdot[m * T]);
             }
         }
     }

@@ -121,6 +121,19 @@ _SIGNATURES = {
     "drmb200_contact_impulse": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
                                                _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int32,
                                                ctypes.c_float, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_contact_backward_workspace_bytes": (ctypes.c_int64, [ctypes.POINTER(Topology), ctypes.c_int32,
+                                                                  ctypes.POINTER(ctypes.c_int32), ctypes.c_int32, ctypes.c_int64]),
+    "drmb200_contact_dynamics_backward": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                                         _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                         _c_float_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint32,
+                                                         ctypes.c_int32, ctypes.c_float, _c_float_p, _c_float_p, _c_float_p,
+                                                         _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
+                                                         ctypes.c_void_p]),
+    "drmb200_contact_impulse_backward": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                                        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_float,
+                                                        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                        ctypes.c_void_p, ctypes.c_void_p]),
     "drmb200_contact_rollout": (ctypes.c_int, [ctypes.POINTER(Topology), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
                                                _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_uint32, ctypes.c_int32,
@@ -589,6 +602,70 @@ def contact_impulse_raw(topo, ee_links, table, q, qd, velocity_ref=None, positio
     return qd_plus, impulse, solved.view(torch.bool)
 
 
+def _contact_workspace(topo, links, position_only, batch, device):
+    nbytes = int(lib().drmb200_contact_backward_workspace_bytes(ctypes.byref(topo), len(links), links,
+                                                               1 if position_only else 0, batch))
+    return torch.empty((max(nbytes, 4) + 3) // 4, device=device, dtype=torch.float32)
+
+
+def contact_dynamics_backward_raw(topo, ee_links, table, q, qd, f, qdd, force, solved, flags, g_qdd=None, g_force=None,
+                                  accel_ref=None, position_only=False, regularization=0.0, want_q=True, want_qd=True,
+                                  want_f=True, want_accel_ref=True, want_table=True):
+    """(q_grad, qd_grad, f_grad [B, n], accel_ref_grad [B, M], table_grad [n_links, 28]) of drmb200_contact_dynamics at the
+    forward's outputs (qdd, force, solved) for the upstream gradients g_qdd [B, n] / g_force [B, M] (None: zero), in at most
+    five launches (drmb200_contact_dynamics_backward); an output not wanted is None.  Unsolved rows get zero gradients."""
+    _require_cuda(table, q, qd, f, qdd, force, g_qdd, g_force, accel_ref)
+    table, q, qd, f, qdd, force = (t.contiguous() for t in (table, q, qd, f, qdd, force))
+    g_qdd, g_force, accel_ref = (None if t is None else t.contiguous() for t in (g_qdd, g_force, accel_ref))
+    solved = solved.contiguous().view(torch.uint8)
+    B, n = q.shape
+    E = len(ee_links)
+    M = (3 if position_only else 6) * E
+    dev = q.device
+    outs = [torch.empty((B, n), device=dev, dtype=torch.float32) if w else None for w in (want_q, want_qd, want_f)]
+    ref_grad = torch.empty((B, M), device=dev, dtype=torch.float32) if want_accel_ref else None
+    table_grad = torch.zeros_like(table) if want_table else None
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    ws = _contact_workspace(topo, links, position_only, B, dev)
+    with _on(dev):
+        rc = lib().drmb200_contact_dynamics_backward(ctypes.byref(topo), E, links, _ptr(table), _ptr(q), _ptr(qd), _ptr(f),
+                                                     _ptr(accel_ref), _ptr(qdd), _ptr(force), _ptr(solved), B, flags & 3,
+                                                     1 if position_only else 0, ctypes.c_float(regularization), _ptr(g_qdd),
+                                                     _ptr(g_force), *[_ptr(t) for t in outs], _ptr(ref_grad), _ptr(table_grad),
+                                                     _ptr(ws), _stream())
+    _check(rc, "drmb200_contact_dynamics_backward")
+    return (*outs, ref_grad, table_grad)
+
+
+def contact_impulse_backward_raw(topo, ee_links, table, q, qd, qd_plus, impulse, solved, g_qd_plus=None, g_impulse=None,
+                                 velocity_ref=None, position_only=False, regularization=0.0, want_q=True, want_qd=True,
+                                 want_velocity_ref=True, want_table=True):
+    """(q_grad, qd_grad [B, n], velocity_ref_grad [B, M], table_grad [n_links, 28]) of drmb200_contact_impulse at the
+    forward's outputs for the upstream gradients g_qd_plus [B, n] / g_impulse [B, M] (None: zero), in at most five launches
+    (drmb200_contact_impulse_backward); an output not wanted is None.  Unsolved rows get zero gradients."""
+    _require_cuda(table, q, qd, qd_plus, impulse, g_qd_plus, g_impulse, velocity_ref)
+    table, q, qd, qd_plus, impulse = (t.contiguous() for t in (table, q, qd, qd_plus, impulse))
+    g_qd_plus, g_impulse, velocity_ref = (None if t is None else t.contiguous() for t in (g_qd_plus, g_impulse, velocity_ref))
+    solved = solved.contiguous().view(torch.uint8)
+    B, n = q.shape
+    E = len(ee_links)
+    M = (3 if position_only else 6) * E
+    dev = q.device
+    outs = [torch.empty((B, n), device=dev, dtype=torch.float32) if w else None for w in (want_q, want_qd)]
+    ref_grad = torch.empty((B, M), device=dev, dtype=torch.float32) if want_velocity_ref else None
+    table_grad = torch.zeros_like(table) if want_table else None
+    links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
+    ws = _contact_workspace(topo, links, position_only, B, dev)
+    with _on(dev):
+        rc = lib().drmb200_contact_impulse_backward(ctypes.byref(topo), E, links, _ptr(table), _ptr(q), _ptr(qd),
+                                                    _ptr(velocity_ref), _ptr(qd_plus), _ptr(impulse), _ptr(solved), B,
+                                                    1 if position_only else 0, ctypes.c_float(regularization), _ptr(g_qd_plus),
+                                                    _ptr(g_impulse), *[_ptr(t) for t in outs], _ptr(ref_grad),
+                                                    _ptr(table_grad), _ptr(ws), _stream())
+    _check(rc, "drmb200_contact_impulse_backward")
+    return (*outs, ref_grad, table_grad)
+
+
 def contact_rollout_raw(topo, ee_links, table, q0, qd0, f, dt, flags, target_pos=None, target_quat=None, position_only=False,
                         regularization=0.0, stabilization=0.0, want_qdd=True, want_force=True, want_accel_ref=False):
     """(q, qd, qdd [T, B, n], force [T, B, M], accel_ref [T, B, M], solved [B] bool) of T semi-implicit Euler steps of the
@@ -1052,6 +1129,63 @@ class PDRolloutFunction(torch.autograd.Function):
         grads = (table_grad, q0_grad, qd0_grad, q_ref_grad, qd_ref_grad, f_grad, kp_grad, kd_grad)
         deps = tuple(t for t in given if t is not None) + (g_q, g_qd, g_qdd, g_tau)
         return first_order_only(grads, deps) + (None,) * 4
+
+
+class ContactDynamicsFunction(torch.autograd.Function):
+    """(table, q, qd, f, accel_ref) -> (qdd, force, solved) of rigid contacts at several links: the single
+    drmb200_contact_dynamics launch forward (the same outputs, bit for bit), drmb200_contact_dynamics_backward backward.
+    ``solved`` is not differentiable; unsolved rows get zero gradients."""
+
+    @staticmethod
+    def forward(ctx, table, q, qd, f, accel_ref, topo, ee_links, flags, position_only, regularization):
+        inputs = (table, q, qd, f, accel_ref)  # as given, not the contiguous copies: first_order_only links to them
+        qdd, force, solved = contact_dynamics_raw(topo, ee_links, table.contiguous(), q, qd, f, flags, accel_ref,
+                                                  position_only, regularization)
+        ctx.save_for_backward(*inputs, qdd, force, solved)
+        ctx.topo, ctx.ee_links, ctx.flags = topo, tuple(ee_links), flags
+        ctx.position_only, ctx.regularization = position_only, regularization
+        ctx.mark_non_differentiable(solved)
+        return qdd, force, solved
+
+    @staticmethod
+    def backward(ctx, g_qdd, g_force, _g_solved):
+        saved = ctx.saved_tensors
+        table, q, qd, f, accel_ref, qdd, force, solved = saved
+        need = ctx.needs_input_grad
+        grads = contact_dynamics_backward_raw(ctx.topo, ctx.ee_links, table, q, qd, f, qdd, force, solved, ctx.flags, g_qdd,
+                                              g_force, accel_ref, ctx.position_only, ctx.regularization, want_q=need[1],
+                                              want_qd=need[2], want_f=need[3], want_accel_ref=need[4], want_table=need[0])
+        q_grad, qd_grad, f_grad, ref_grad, table_grad = grads
+        return first_order_only((table_grad, q_grad, qd_grad, f_grad, ref_grad),
+                                saved[:5] + (g_qdd, g_force)) + (None,) * 5
+
+
+class ContactImpulseFunction(torch.autograd.Function):
+    """(table, q, qd, velocity_ref) -> (qd_plus, impulse, solved) of an impact at several links: the single
+    drmb200_contact_impulse launch forward (the same outputs, bit for bit), drmb200_contact_impulse_backward backward.
+    ``solved`` is not differentiable; unsolved rows get zero gradients."""
+
+    @staticmethod
+    def forward(ctx, table, q, qd, velocity_ref, topo, ee_links, position_only, regularization):
+        inputs = (table, q, qd, velocity_ref)  # as given, not the contiguous copies: first_order_only links to them
+        qd_plus, impulse, solved = contact_impulse_raw(topo, ee_links, table.contiguous(), q, qd, velocity_ref, position_only,
+                                                       regularization)
+        ctx.save_for_backward(*inputs, qd_plus, impulse, solved)
+        ctx.topo, ctx.ee_links = topo, tuple(ee_links)
+        ctx.position_only, ctx.regularization = position_only, regularization
+        ctx.mark_non_differentiable(solved)
+        return qd_plus, impulse, solved
+
+    @staticmethod
+    def backward(ctx, g_qd_plus, g_impulse, _g_solved):
+        saved = ctx.saved_tensors
+        table, q, qd, velocity_ref, qd_plus, impulse, solved = saved
+        need = ctx.needs_input_grad
+        q_grad, qd_grad, ref_grad, table_grad = contact_impulse_backward_raw(
+            ctx.topo, ctx.ee_links, table, q, qd, qd_plus, impulse, solved, g_qd_plus, g_impulse, velocity_ref,
+            ctx.position_only, ctx.regularization, want_q=need[1], want_qd=need[2], want_velocity_ref=need[3],
+            want_table=need[0])
+        return first_order_only((table_grad, q_grad, qd_grad, ref_grad), saved[:4] + (g_qd_plus, g_impulse)) + (None,) * 4
 
 
 def mass_matrix_raw(topo, table, q, out=None, folded=None):

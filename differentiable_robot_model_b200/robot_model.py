@@ -665,6 +665,7 @@ class DifferentiableRobotModel(torch.nn.Module):
         use_damping: Optional[bool] = False,
         position_only: bool = False,
         regularization: float = 0.0,
+        differentiable: bool = False,
     ) -> ContactDynamics:
         r"""Forward dynamics with the links held by bilateral rigid contacts (at most 8, distinct), in ONE launch
         (``csrc/contact_dynamics.cu``; the definition and the solve are stated in ``include/drm_b200.h``).  With ``J``, ``G``,
@@ -683,14 +684,24 @@ class DifferentiableRobotModel(torch.nn.Module):
             include_gravity, use_damping: as for :meth:`compute_forward_dynamics`
             position_only: hold the link origins only (3 rows per link) instead of the full pose (6)
             regularization: ``mu >= 0``; redundant constraint sets (more rows than the joints can satisfy) need ``mu > 0``
+            differentiable: make ``qdd`` and ``force`` differentiable (see below); off by default
         Returns: :class:`ContactDynamics` ``(qdd, force, solved)``, squeezed for 1-D inputs.  A row whose equilibrated system
-        has a pivot of magnitude <= 1e-5 is not solved: ``solved`` is False and its outputs are NaN.  The outputs carry no
-        autograd graph: they use the current values of the link parameters (learnable and fused ones included) but are not
-        differentiable."""
+        has a pivot of magnitude <= 1e-5 is not solved: ``solved`` is False and its outputs are NaN.  By default the outputs
+        carry no autograd graph: they use the current values of the link parameters (learnable and fused ones included) but
+        are not differentiable.
+
+        With ``differentiable=True``, grad mode on and any of q, qd, f, accel_ref or a learnable link parameter requiring
+        grad, ``qdd`` and ``force`` are differentiable w.r.t. all of them (fused parameters included) through the analytic
+        adjoint (``csrc/contact_backward.cu``, stated in ``include/drm_b200.h``): for upstream gradients ``g_qdd``,
+        ``g_force``, ``nu`` solves ``A^T nu = g_force + J G^T g_qdd``, ``accel_ref`` receives ``nu``, and q, qd, f and the link
+        parameters receive the forward-dynamics adjoint at ``(q, qd, f + J^T lambda)`` for ``g_qdd - J^T nu`` plus the
+        derivatives of ``lambda^T J f_grad - nu^T (J qdd + Jdot qd)``.  Unsolved rows receive exactly zero gradients,
+        whatever their upstream gradient.  ``regularization`` is not differentiated, ``solved`` carries no graph, and the
+        gradients are first-order only.  The forward is the same single launch with the same outputs, bit for bit."""
         links = self._contact_links(link_names)
         out = self._contact_dynamics(q, qd, f, accel_ref, links=links, include_gravity=include_gravity,
                                      use_damping=use_damping, position_only=bool(position_only),
-                                     regularization=float(regularization))
+                                     regularization=float(regularization), differentiable=bool(differentiable))
         return ContactDynamics(*out)
 
     def compute_contact_impulse(
@@ -701,6 +712,7 @@ class DifferentiableRobotModel(torch.nn.Module):
         velocity_ref: Optional[torch.Tensor] = None,
         position_only: bool = False,
         regularization: float = 0.0,
+        differentiable: bool = False,
     ) -> ContactImpulse:
         r"""The joint velocities after an instantaneous impact at the links (at most 8, distinct), in ONE launch
         (``csrc/contact_dynamics.cu``; stated in ``include/drm_b200.h``).  With ``J`` and ``G`` as in
@@ -717,11 +729,19 @@ class DifferentiableRobotModel(torch.nn.Module):
             q, qd: joint angles / velocities before the impact [batch_size x n_dofs]
             link_names, position_only, regularization: as for :meth:`compute_contact_dynamics`
             velocity_ref: the desired constraint-space velocity after the impact [batch_size x M]; None: 0
+            differentiable: make ``qd_plus`` and ``impulse`` differentiable (see below); off by default
         Returns: :class:`ContactImpulse` ``(qd_plus, impulse, solved)``, squeezed for 1-D inputs; unsolved rows as in
-        :meth:`compute_contact_dynamics`.  No autograd graph, current link parameters."""
+        :meth:`compute_contact_dynamics`.  By default no autograd graph, current link parameters.
+
+        With ``differentiable=True``, grad mode on and any of q, qd, velocity_ref or a learnable link parameter requiring
+        grad, ``qd_plus`` and ``impulse`` are differentiable w.r.t. all of them: as for :meth:`compute_contact_dynamics`,
+        with ``nu`` solving ``A^T nu = g_impulse + J G^T g_qd_plus``, ``velocity_ref`` receiving ``nu``, qd receiving
+        ``g_qd_plus - J^T nu``, and q and the link parameters the forward-dynamics adjoint at ``(q, 0, J^T Lambda)`` plus the
+        derivatives of ``Lambda^T J tau - nu^T J qd_plus``.  Unsolved rows receive exactly zero gradients; ``regularization``
+        is not differentiated; ``solved`` carries no graph; first-order only; the forward is the same launch, bit for bit."""
         links = self._contact_links(link_names)
         out = self._contact_impulse(q, qd, velocity_ref, links=links, position_only=bool(position_only),
-                                    regularization=float(regularization))
+                                    regularization=float(regularization), differentiable=bool(differentiable))
         return ContactImpulse(*out)
 
     def _contact_links(self, link_names):
@@ -730,21 +750,32 @@ class DifferentiableRobotModel(torch.nn.Module):
         return links
 
     @tensor_check
-    def _contact_dynamics(self, q, qd, f, accel_ref, links, include_gravity, use_damping, position_only, regularization):
+    def _contact_dynamics(self, q, qd, f, accel_ref, links, include_gravity, use_damping, position_only, regularization,
+                          differentiable=False):
         self._check_q(q, qd, f)
         M = (3 if position_only else 6) * len(links)
         assert accel_ref is None or tuple(accel_ref.shape) == (q.shape[0], M), f"accel_ref must be [batch_size x {M}]"
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
-        table = self._link_table().detach()
+        table = self._link_table()
+        if differentiable and torch.is_grad_enabled() and any(t is not None and t.requires_grad
+                                                              for t in (table, q, qd, f, accel_ref)):
+            return engine.ContactDynamicsFunction.apply(table, q, qd, f, accel_ref, self._topology, links, flags, position_only,
+                                                        regularization)
+        table = table.detach()
         return engine.contact_dynamics_raw(self._topology, links, table, q.detach(), qd.detach(), f.detach(), flags,
                                            None if accel_ref is None else accel_ref.detach(), position_only, regularization)
 
     @tensor_check
-    def _contact_impulse(self, q, qd, velocity_ref, links, position_only, regularization):
+    def _contact_impulse(self, q, qd, velocity_ref, links, position_only, regularization, differentiable=False):
         self._check_q(q, qd)
         M = (3 if position_only else 6) * len(links)
         assert velocity_ref is None or tuple(velocity_ref.shape) == (q.shape[0], M), f"velocity_ref must be [batch_size x {M}]"
-        table = self._link_table().detach()
+        table = self._link_table()
+        if differentiable and torch.is_grad_enabled() and any(t is not None and t.requires_grad
+                                                              for t in (table, q, qd, velocity_ref)):
+            return engine.ContactImpulseFunction.apply(table, q, qd, velocity_ref, self._topology, links, position_only,
+                                                       regularization)
+        table = table.detach()
         return engine.contact_impulse_raw(self._topology, links, table, q.detach(), qd.detach(),
                                           None if velocity_ref is None else velocity_ref.detach(), position_only, regularization)
 

@@ -31,7 +31,8 @@
  *                                        accelerations of several links, one launch (the reference has none of these).
  *   drmb200_contact_dynamics / drmb200_contact_impulse   joint accelerations and contact forces under rigid contacts at
  *                                        several links, and the joint velocities and impulses of an impact there, one launch
- *                                        each (the reference has none of these).
+ *                                        each (the reference has none of these); drmb200_contact_dynamics_backward /
+ *                                        drmb200_contact_impulse_backward are their analytic adjoints.
  *   drmb200_contact_rollout              T semi-implicit Euler steps of the contact dynamics with Baumgarte stabilisation
  *                                        towards fixed link targets, one launch (the reference has none of these).
  *   drmb200_dynamics_regressor           the joint-torque regressor Y, tau = Y . (I_o, mc, m, damping of every link), one
@@ -517,6 +518,53 @@ int drmb200_contact_impulse(const drmb200_topology_t* topo, int32_t n_ee, const 
                             const float* q, const float* qd, const float* velocity_ref, int64_t batch,
                             int32_t position_only, float regularization,
                             float* qd_plus, float* impulse, uint8_t* solved, void* cuda_stream);
+
+/*
+ * Adjoints of drmb200_contact_dynamics and drmb200_contact_impulse (csrc/contact_backward.cu).  Given the forward's inputs, its
+ * outputs qdd / qd_plus [B, n], force / impulse [B, M] and solved [B], and the upstream gradients g_qdd / g_qd_plus [B, n]
+ * and g_force / g_impulse [B, M] (NULL: zero), per row, with J, G, A = J G J^T + mu I and qdd_free as stated above:
+ *   lambda is defined implicitly by qdd = FD(q, qd, tau_c), tau_c = f + J^T lambda, and J qdd + Jdot qd = a_ref - mu lambda.
+ *   Differentiating that equation:
+ *     s      = g_force + J G^T g_qdd                  (G is not assumed symmetric)
+ *     nu     solves A^T nu = s
+ *     g^     = g_qdd - J^T nu;                        accel_ref_grad = nu
+ *     (q1, qd1, theta1, tau^) = the adjoint of drmb200_forward_dynamics at (q, qd, tau_c) with upstream g^, the call's flags;
+ *                                                      f_grad = tau^
+ *     phi(q, qd; theta) = lambda^T J(q) tau^ - nu^T (J(q) qdd + Jdot(q, qd) qd)   with lambda, nu, tau^, qdd held constant
+ *     q_grad = q1 + dphi/dq,  qd_grad = qd1 + dphi/dqd,  table_grad += theta1 + dphi/dtheta (the kinematic F, r columns)
+ *   The impulse is the same with qdd -> qd_plus and lambda -> Lambda: the forward-dynamics adjoint runs at (q, 0, J^T Lambda)
+ *   without flags, phi has no Jdot term (J qd_plus only), qd_grad = g^ and velocity_ref_grad = nu.
+ * A^T nu = s is solved on the forward's factorisation: with S = diag(|A_kk|^-1/2), A~ = S A S and P A~ = L U by the forward's
+ * elimination (the same float operations, so the same pivots and the same solved decision, bit for bit), A~^T y = S s and
+ * nu = S y.  mu is not differentiated.  A row contributes only when the forward's solved[b] is set and the backward's own
+ * factorisation (which repeats the forward's, so it decides the same) succeeds; every other row contributes exactly zero
+ * to every gradient, whatever its upstream gradient and even when its inputs are not finite: its q_grad, qd_grad, f_grad,
+ * accel_ref_grad / velocity_ref_grad rows are 0 and it adds nothing to table_grad.
+ * Outputs, caller-allocated, fp32, must not alias inputs; each may be NULL: q_grad, qd_grad, f_grad [B, n],
+ * accel_ref_grad / velocity_ref_grad [B, M], and table_grad [n_links, 28], which is ACCUMULATED into (a sum over the batch,
+ * bitwise reproducible).  `workspace` must hold drmb200_contact_backward_workspace_bytes(topo, n_ee, ee_links,
+ * position_only, batch) bytes.  Three stages in stream order: one launch of the contact adjoint kernel (nu, g^, tau_c); then,
+ * when any of q_grad, qd_grad, f_grad, table_grad is wanted, the forward-dynamics adjoint (one launch, plus its reduction
+ * with table_grad); then, when any of q_grad, qd_grad (dynamics only) or table_grad is wanted, one launch of the kinematic
+ * adjoint kernel (plus its reduction with table_grad).  At most 5 launches; nothing is allocated or synchronised
+ * (graph-capturable).  batch == 0 is a no-op.  Errors: those of the forward (checked before any launch), a null required
+ * pointer (batch > 0) or workspace; DRMB200_ELIMIT, naming the bytes, when one row of either adjoint kernel needs more than
+ * 227 KB of shared memory.
+ */
+int64_t drmb200_contact_backward_workspace_bytes(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links,
+                                                 int32_t position_only, int64_t batch);
+int drmb200_contact_dynamics_backward(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                      const float* q, const float* qd, const float* f, const float* accel_ref, const float* qdd,
+                                      const float* force, const uint8_t* solved, int64_t batch, uint32_t flags,
+                                      int32_t position_only, float regularization, const float* g_qdd, const float* g_force,
+                                      float* q_grad, float* qd_grad, float* f_grad, float* accel_ref_grad, float* table_grad,
+                                      void* workspace, void* cuda_stream);
+int drmb200_contact_impulse_backward(const drmb200_topology_t* topo, int32_t n_ee, const int32_t* ee_links, const float* table,
+                                     const float* q, const float* qd, const float* velocity_ref, const float* qd_plus,
+                                     const float* impulse, const uint8_t* solved, int64_t batch, int32_t position_only,
+                                     float regularization, const float* g_qd_plus, const float* g_impulse, float* q_grad,
+                                     float* qd_grad, float* velocity_ref_grad, float* table_grad, void* workspace,
+                                     void* cuda_stream);
 
 /*
  * Contact-constrained rollouts: T steps of semi-implicit Euler over drmb200_contact_dynamics with Baumgarte stabilisation,
