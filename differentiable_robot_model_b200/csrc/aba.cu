@@ -42,11 +42,12 @@ struct AbaArgs {
     int64_t batch;
     uint32_t flags;
     int32_t aligned;
+    float h;                        // IMPLICIT: the step of the implicit damping
 };
 
-template <int T>
-__global__ void __launch_bounds__(T)
-aba_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const AbaArgs args) {
+// The kernel's body, instantiated by aba_kernel and aba_implicit_kernel (IMPLICIT: implicit damping of step args.h)
+template <int T, bool IMPLICIT>
+__device__ __forceinline__ void aba_run(const TreeProgram& prog, const FoldProgram& fold, const AbaArgs args) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar;
 
@@ -95,8 +96,8 @@ aba_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ Fol
     if (bulk) mbar_wait(&mbar, 0);
 
     if (tid < valid)
-        aba_body<T>(prog, s_tab, s_q + tid * n, s_qd + tid * n, s_f + tid * n, s_qdd + tid * n, s_link + tid, s_slot + tid,
-                    args.flags);
+        aba_body<T, IMPLICIT>(prog, s_tab, s_q + tid * n, s_qd + tid * n, s_f + tid * n, s_qdd + tid * n, s_link + tid,
+                              s_slot + tid, args.flags, args.h);
 
     if (bulk) {
         fence_proxy_async();
@@ -112,12 +113,24 @@ aba_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ Fol
     }
 }
 
+template <int T>
+__global__ void __launch_bounds__(T)
+aba_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const AbaArgs args) {
+    aba_run<T, false>(prog, fold, args);
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+aba_implicit_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const AbaArgs args) {
+    aba_run<T, true>(prog, fold, args);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 static int forward_dynamics_device_impl(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                                        const float* f, int64_t batch, uint32_t flags, float* qdd, cudaStream_t stream,
-                                       bool prefolded) {
+                                       bool prefolded, float dt) {
     FoldChoice fc;
     const int rc = select_fold(topo, prefolded, &fc);
     if (rc != DRMB200_OK) return rc;
@@ -128,6 +141,7 @@ static int forward_dynamics_device_impl(const drmb200_topology_t* topo, const fl
 
     AbaArgs args;
     args.table = table; args.q = q; args.qd = qd; args.f = f; args.qdd = qdd; args.batch = batch; args.flags = flags;
+    args.h = dt;
     args.aligned = aligned16(q, qd, f, qdd);
 
     // 64 configurations per CTA unless the model's per-link state would leave a single CTA per SM
@@ -136,17 +150,30 @@ static int forward_dynamics_device_impl(const drmb200_topology_t* topo, const fl
     });
     if (c.bytes > SMEM_CTA_MAX) { set_error("model needs %zu B of shared memory per CTA (> 227 KB)", c.bytes); return DRMB200_ELIMIT; }
     const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    if (flags & DRMB200_IMPLICIT_DAMPING)
+        return c.tile == 64 ? launch_kernel<aba_implicit_kernel<64>>(tiles, 64, c.bytes, stream, false, "aba", prog, fc.fold, args)
+                            : launch_kernel<aba_implicit_kernel<32>>(tiles, 32, c.bytes, stream, false, "aba", prog, fc.fold, args);
     return c.tile == 64 ? launch_kernel<aba_kernel<64>>(tiles, 64, c.bytes, stream, false, "aba", prog, fc.fold, args)
                         : launch_kernel<aba_kernel<32>>(tiles, 32, c.bytes, stream, false, "aba", prog, fc.fold, args);
 }
 
 int forward_dynamics_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                             const float* f, int64_t batch, uint32_t flags, float* qdd, cudaStream_t stream) {
-    return forward_dynamics_device_impl(topo, table, q, qd, f, batch, flags, qdd, stream, false);
+    return forward_dynamics_device_impl(topo, table, q, qd, f, batch, flags & ~DRMB200_IMPLICIT_DAMPING, qdd, stream, false,
+                                        0.f);
 }
 int forward_dynamics_prefolded_device(const drmb200_topology_t* topo, const float* folded, const float* q, const float* qd,
                                       const float* f, int64_t batch, uint32_t flags, float* qdd, cudaStream_t stream) {
-    return forward_dynamics_device_impl(topo, folded, q, qd, f, batch, flags, qdd, stream, true);
+    return forward_dynamics_device_impl(topo, folded, q, qd, f, batch, flags & ~DRMB200_IMPLICIT_DAMPING, qdd, stream, true,
+                                        0.f);
+}
+int forward_dynamics_implicit_damping_device(const drmb200_topology_t* topo, const float* table, const float* q,
+                                             const float* qd, const float* f, int64_t batch, uint32_t flags, float dt,
+                                             float* qdd, cudaStream_t stream) {
+    flags |= DRMB200_IMPLICIT_DAMPING;
+    const int rc = check_implicit_damping(flags, dt);
+    if (rc != DRMB200_OK) return rc;
+    return forward_dynamics_device_impl(topo, table, q, qd, f, batch, flags, qdd, stream, false, dt);
 }
 
 }  // namespace drm

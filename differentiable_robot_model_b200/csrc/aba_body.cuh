@@ -142,9 +142,13 @@ __device__ __forceinline__ void sub_outer_pp(M3PP& m, V3 x, const V3P& yp) {
 
 // One configuration (one thread): qdd of row `qrow` / `qdrow` / `frow` into `outrow`.  s_tab holds the staged canonical
 // (possibly folded) table; lk0 / sl0 are this thread's column of the per-link and branch-slot regions (stride T).
-template <int T>
+// IMPLICIT: implicit joint damping with step h (include/drm_b200.h) -- every movable joint's pivot d = S^T IA S becomes
+// d + h damping wherever it is used (passes 2 and 3 here, and the unit-response sweeps that read the stored d), which gives
+// (H + h diag(damping))^-1 (f - nle) for symmetric inertias.  The damping torque itself still needs DRMB200_DAMPING.
+template <int T, bool IMPLICIT = false>
 __device__ __forceinline__ void aba_body(const TreeProgram& prog, const float* s_tab, const float* qrow, const float* qdrow,
-                                         const float* frow, float* outrow, float* lk0, float* sl0, uint32_t flags) {
+                                         const float* frow, float* outrow, float* lk0, float* sl0, uint32_t flags,
+                                         float h = 0.f) {
     const int N = prog.n_links;
     const float g = (flags & DRMB200_GRAVITY) ? ABA_GRAVITY : 0.f;
     const bool damp = (flags & DRMB200_DAMPING) != 0;
@@ -216,6 +220,7 @@ __device__ __forceinline__ void aba_body(const TreeProgram& prog, const float* s
                 upk2(AB.a02, Ua.x, t); upk2(AB.a12, Ua.y, t); upk2(AB.a22, Ua.z, t);    // U = IA S, S = e_z(ang)   (:555)
                 upk2(CD.a02, Ul.x, t); upk2(CD.a12, Ul.y, t); upk2(CD.a22, Ul.z, t);
                 d = Ua.z;                                                      // S . U                    (:557)
+                if constexpr (IMPLICIT) d = fmaf(h, C.d, d);                   // + h damping
                 float fk = frow[c];
                 if (damp) fk = fmaf(-C.d, qdrow[c], fk);                       // f -= damping * qd        (:516-521)
                 u = fk - p_ang.z;                                              // (:559)

@@ -45,6 +45,7 @@ struct AbaBwdArgs {
     uint32_t flags;
     int32_t vec_ok;
     int32_t accumulate;                // add to the per-CTA partial tables instead of overwriting them
+    float h;                           // IMPLICIT: the step of the implicit damping
 };
 
 struct AbaBwdSmem {
@@ -145,7 +146,9 @@ __device__ __forceinline__ void st_blocks(float* p, int T, const Blocks& b) {
     stm(p, T, b.A); stm(p + 9 * T, T, b.B); stm(p + 18 * T, T, b.C); stm(p + 27 * T, T, b.D);
 }
 
-template <bool NEED_TABLE, int T>
+// IMPLICIT: the adjoint of aba_body<T, true> -- every use of Ua.z as the pivot becomes Ua.z + h damping, and the pivot's
+// adjoint d-bar also reaches the damping column of the table (h d-bar, on top of the damping torque's -u-bar qd).
+template <bool NEED_TABLE, int T, bool IMPLICIT = false>
 __global__ void __launch_bounds__(T < 32 ? 32 : T)
 aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs args) {
     constexpr int TB = T < 32 ? 32 : T;
@@ -168,6 +171,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
     const bool vec_ok = args.vec_ok;
     const float grav = (args.flags & DRMB200_GRAVITY) ? GRAVITY_B : 0.f;
     const bool damp = (args.flags & DRMB200_DAMPING) != 0;
+    auto pivot = [&](float uz, int i) { return IMPLICIT ? fmaf(args.h, s_tab[i * DRMB200_TABLE_STRIDE + 25], uz) : uz; };
 
     for (int i = tid; i < N * DRMB200_TABLE_STRIDE; i += TB) {
         const int l = i / DRMB200_TABLE_STRIDE, e = i - l * DRMB200_TABLE_STRIDE;
@@ -243,7 +247,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
             V3 Ua = zero, Ul = zero;
             float d = 0.f, u = 0.f;
             if (c >= 0) {
-                Ua = col2(I.A); Ul = col2(I.C); d = Ua.z;
+                Ua = col2(I.A); Ul = col2(I.C); d = pivot(Ua.z, i);
                 float fk = frow[c];
                 if (damp) fk = fmaf(-s_tab[i * DRMB200_TABLE_STRIDE + 25], qdrow[c], fk);
                 u = fk - pa_ang.z;
@@ -301,7 +305,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
                 al = al + cross_z(w, qd_k); a = a + cross_z(v, qd_k);
                 const V3 Ua = v3(gia0[(i * IA_FLOATS + 2) * T], gia0[(i * IA_FLOATS + 5) * T], gia0[(i * IA_FLOATS + 8) * T]);
                 const V3 Ul = v3(gia0[(i * IA_FLOATS + 20) * T], gia0[(i * IA_FLOATS + 23) * T], gia0[(i * IA_FLOATS + 26) * T]);
-                const float qdd = (1.0f / Ua.z) * (lk[O_U * T] - (dot(Ua, al) + dot(Ul, a)));
+                const float qdd = (1.0f / pivot(Ua.z, i)) * (lk[O_U * T] - (dot(Ua, al) + dot(Ul, a)));
                 al.z += qdd;
             }
             if (writer) { stv(lk + O_AL * T, T, al); stv(lk + (O_AL + 3) * T, T, a); }
@@ -326,7 +330,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
                 const V3 aq = mulT(M, cross_add(alp, r, ap)) + cross_z(v, qd_k);
                 const V3 Ua = v3(gia0[(i * IA_FLOATS + 2) * T], gia0[(i * IA_FLOATS + 5) * T], gia0[(i * IA_FLOATS + 8) * T]);
                 const V3 Ul = v3(gia0[(i * IA_FLOATS + 20) * T], gia0[(i * IA_FLOATS + 23) * T], gia0[(i * IA_FLOATS + 26) * T]);
-                const float dinv = 1.0f / Ua.z;
+                const float dinv = 1.0f / pivot(Ua.z, i);
                 const float qdd = dinv * (lk[O_U * T] - (dot(Ua, alq) + dot(Ul, aq)));
                 const float k = (grow[c] + alq_b.z) * dinv;
                 if (writer) {
@@ -395,7 +399,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
                 float inv = 0.f, u = 0.f;
                 V3 ca = zero, cl = zero;
                 if (c >= 0) {
-                    inv = 1.f / (Ua.z + ABA_EPS_B);
+                    inv = 1.f / (pivot(Ua.z, i) + ABA_EPS_B);
                     u = lk[O_U * T];
                     const V3 Uda = inv * Ua, Udl = inv * Ul;
                     sub_outer_b(I.A, Ua, Uda); sub_outer_b(I.B, Ua, Udl); sub_outer_b(I.C, Ul, Uda); sub_outer_b(I.D, Ul, Udl);
@@ -467,6 +471,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
                 if (damp) {
                     if (writer) qdg[c] = fmaf(-s_tab[i * DRMB200_TABLE_STRIDE + 25], ub, qdg[c]);
                     vals[25] = -ub * qdrow[c];
+                    if constexpr (IMPLICIT) vals[25] = fmaf(args.h, db, vals[25]);      // d = Ua.z + h damping
                 }
                 pb_ang.z -= ub;
                 Uab.z += db;
@@ -571,11 +576,12 @@ int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t* topo
 
 // accumulate_partials / reduce: a caller that runs the adjoint several times on batches of the same size (the steps of a
 // rollout, rollout.cu) can sum the per-CTA partial tables of all calls in the workspace and reduce them into table_grad once,
-// with the last call; the default (false, true) is one self-contained adjoint.
+// with the last call; the default (false, true) is one self-contained adjoint.  With DRMB200_IMPLICIT_DAMPING in flags,
+// the adjoint of the forward dynamics with implicit damping of step dt (checked by the caller).
 int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                                      const float* f, int64_t batch, uint32_t flags, const float* g_qdd,
                                      float* q_grad, float* qd_grad, float* f_grad, float* table_grad, void* workspace,
-                                     cudaStream_t stream, bool accumulate_partials, bool reduce) {
+                                     cudaStream_t stream, bool accumulate_partials, bool reduce, float dt) {
     TreeProgram prog;
     int rc = build_tree_program(topo, &prog);
     if (rc != DRMB200_OK) return rc;
@@ -592,6 +598,7 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     args.scratch = reinterpret_cast<float*>(static_cast<char*>(workspace) + table_grad_workspace_bytes(topo, batch));
     args.batch = batch; args.flags = flags;
     args.accumulate = accumulate_partials ? 1 : 0;
+    args.h = dt;
     args.vec_ok = aligned16(q, qd, f, g_qdd, q_grad, qd_grad, f_grad);
 
     auto bytes_of = [&](int t) { return (size_t)AbaBwdSmem(t, prog.n_dofs, prog.n_links).total_floats * sizeof(float); };
@@ -601,10 +608,15 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     const int64_t tiles = (batch + tile - 1) / tile;
     int grid = 0;
     const bool need_table = table_grad != nullptr;
-#define DRM_LAUNCH_ABAB(NT, TT) \
-    rc = launch_persistent<aba_backward_kernel<NT, TT>>(TT < 32 ? 32 : TT, smem_bytes, tiles, stream, "aba backward", &grid, prog, args)
-    if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB(true, 32); else DRM_LAUNCH_ABAB(true, 16); }
-    else            { if (tile == 32) DRM_LAUNCH_ABAB(false, 32); else DRM_LAUNCH_ABAB(false, 16); }
+#define DRM_LAUNCH_ABAB(NT, TT, IM) \
+    rc = launch_persistent<aba_backward_kernel<NT, TT, IM>>(TT < 32 ? 32 : TT, smem_bytes, tiles, stream, "aba backward", &grid, prog, args)
+    if (flags & DRMB200_IMPLICIT_DAMPING) {
+        if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB(true, 32, true); else DRM_LAUNCH_ABAB(true, 16, true); }
+        else            { if (tile == 32) DRM_LAUNCH_ABAB(false, 32, true); else DRM_LAUNCH_ABAB(false, 16, true); }
+    } else {
+        if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB(true, 32, false); else DRM_LAUNCH_ABAB(true, 16, false); }
+        else            { if (tile == 32) DRM_LAUNCH_ABAB(false, 32, false); else DRM_LAUNCH_ABAB(false, 16, false); }
+    }
 #undef DRM_LAUNCH_ABAB
     if (rc != DRMB200_OK) return rc;
     return need_table && reduce ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
@@ -614,8 +626,19 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
                                      const float* f, int64_t batch, uint32_t flags, const float* g_qdd,
                                      float* q_grad, float* qd_grad, float* f_grad, float* table_grad, void* workspace,
                                      cudaStream_t stream) {
+    return forward_dynamics_backward_device(topo, table, q, qd, f, batch, flags & ~DRMB200_IMPLICIT_DAMPING, g_qdd, q_grad,
+                                            qd_grad, f_grad, table_grad, workspace, stream, false, true, 0.f);
+}
+
+int forward_dynamics_implicit_damping_backward_device(const drmb200_topology_t* topo, const float* table, const float* q,
+                                                      const float* qd, const float* f, int64_t batch, uint32_t flags, float dt,
+                                                      const float* g_qdd, float* q_grad, float* qd_grad, float* f_grad,
+                                                      float* table_grad, void* workspace, cudaStream_t stream) {
+    flags |= DRMB200_IMPLICIT_DAMPING;
+    const int rc = check_implicit_damping(flags, dt);
+    if (rc != DRMB200_OK) return rc;
     return forward_dynamics_backward_device(topo, table, q, qd, f, batch, flags, g_qdd, q_grad, qd_grad, f_grad, table_grad,
-                                            workspace, stream, false, true);
+                                            workspace, stream, false, true, dt);
 }
 
 }  // namespace drm

@@ -96,6 +96,11 @@ int forward_dynamics_device(const drmb200_topology_t*, const float*, const float
                             int64_t, uint32_t, float*, cudaStream_t);
 int forward_dynamics_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*,
                                      int64_t, uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t);
+int forward_dynamics_implicit_damping_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*,
+                                             int64_t, uint32_t, float, float*, cudaStream_t);
+int forward_dynamics_implicit_damping_backward_device(const drmb200_topology_t*, const float*, const float*, const float*,
+                                                      const float*, int64_t, uint32_t, float, const float*, float*, float*,
+                                                      float*, float*, void*, cudaStream_t);
 int forward_dynamics_rollout_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
                                     int32_t, float, uint32_t, float*, float*, float*, cudaStream_t);
 int64_t forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
@@ -393,6 +398,22 @@ int drmb200_forward_dynamics_backward(const drmb200_topology_t* topo, const floa
                                       float* table_grad, void* workspace, void* cuda_stream) {
     return drm::forward_dynamics_backward_device(topo, table, q, qd, f, batch, flags, g_qdd, q_grad, qd_grad, f_grad,
                                                  table_grad, workspace, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_forward_dynamics_implicit_damping(const drmb200_topology_t* topo, const float* table, const float* q,
+                                              const float* qd, const float* f, int64_t batch, uint32_t flags, float dt,
+                                              float* qdd, void* cuda_stream) {
+    return drm::forward_dynamics_implicit_damping_device(topo, table, q, qd, f, batch, flags, dt, qdd,
+                                                         static_cast<cudaStream_t>(cuda_stream));
+}
+
+int drmb200_forward_dynamics_implicit_damping_backward(const drmb200_topology_t* topo, const float* table, const float* q,
+                                                       const float* qd, const float* f, int64_t batch, uint32_t flags,
+                                                       float dt, const float* g_qdd, float* q_grad, float* qd_grad,
+                                                       float* f_grad, float* table_grad, void* workspace, void* cuda_stream) {
+    return drm::forward_dynamics_implicit_damping_backward_device(topo, table, q, qd, f, batch, flags, dt, g_qdd, q_grad,
+                                                                  qd_grad, f_grad, table_grad, workspace,
+                                                                  static_cast<cudaStream_t>(cuda_stream));
 }
 
 int drmb200_forward_dynamics_rollout(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0,

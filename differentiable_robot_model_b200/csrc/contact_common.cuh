@@ -129,7 +129,8 @@ __device__ __forceinline__ void contact_solve_transposed(const float* A, float* 
 //   3. osd_inverse_inertia: A = J G J^T, then MU on the diagonal;
 //   4. contact_solve: lambda, or unsolved;
 //   5. + G J^T lambda (one more aba_unit_response); unsolved rows get NaN in out and lam.
-// OK (a bool lvalue) receives whether the row was solved.  The slots come from the enclosing scope's layout L: the ABA rows
+// OK (a bool lvalue) receives whether the row was solved.  IMPLICIT (a constant) and H: aba_body's implicit damping of step H
+// (dynamics only), which the unit-response sweeps then follow through the stored pivots.  The slots come from the enclosing scope's layout L: the ABA rows
 // s_q / s_qd / s_f / s_qdd (row-major n floats; the f row is overwritten by the unit-response sweeps, the qdd row is
 // scratch), the reference rows (L.ref, row-major M), and slot-major the ABA link and branch state (L.aba.link,
 // L.aba.slots), J [M][n_u] (L.jac), the walk's joint scratch and spilled state (L.jscr, L.state), J qd and Jdot qd (L.vel,
@@ -139,7 +140,7 @@ __device__ __forceinline__ void contact_solve_transposed(const float* A, float* 
 //
 // A macro rather than a __forceinline__ function: a function is simplified on its own before it is inlined, which changes
 // the contact kernel's code generation (its SASS, not its results); the macro expands to the kernel's own statements.
-#define DRM_CONTACT_ROW(T, IMPULSE, POSES, POSE, FLAGS, MU, OK, AFTER_WALK)                                                \
+#define DRM_CONTACT_ROW(T, IMPULSE, POSES, POSE, FLAGS, MU, OK, IMPLICIT, H, AFTER_WALK)                                    \
     do {                                                                                                                   \
         const float* qrow = s_q + tid * n;                                                                                 \
         const float* qdrow = s_qd + tid * n;                                                                               \
@@ -158,7 +159,7 @@ __device__ __forceinline__ void contact_solve_transposed(const float* A, float* 
         osd_walk<T, POSES>(P, s_tab, qrow, qdrow, MR, J, vel, bias, smem + L.jscr + tid, smem + L.state + tid, POSE);      \
         AFTER_WALK                                                                                                         \
         if (!IMPULSE) {                                                                                                    \
-            aba_body<T>(prog, s_tab, qrow, qdrow, frow, xrow, lk0, sl0, FLAGS);                                            \
+            aba_body<T, IMPLICIT>(prog, s_tab, qrow, qdrow, frow, xrow, lk0, sl0, FLAGS, H);                               \
             for (int m = 0; m < M; ++m) { /* a_ref - (J qdd_free + Jdot qd) */                                             \
                 float s = bias[m * T];                                                                                     \
                 for (int u = 0; u < n_u; ++u) s = fmaf(J[m * rs + u * T], xrow[P.u_dof[u]], s);                            \

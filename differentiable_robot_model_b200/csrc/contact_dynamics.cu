@@ -118,7 +118,7 @@ contact_dynamics_kernel(const __grid_constant__ TreeProgram prog, const __grid_c
 
     if (tid < valid) {
         bool ok;
-        DRM_CONTACT_ROW(T, IMPULSE, false, nullptr, args.flags, args.mu, ok, );
+        DRM_CONTACT_ROW(T, IMPULSE, false, nullptr, args.flags, args.mu, ok, false, 0.f, );
         args.solved[tile_start + tid] = ok ? 1 : 0;
     }
     __syncthreads();

@@ -12,7 +12,9 @@
 // With omega = 0 the trajectory is bit-identical to a loop of drmb200_contact_dynamics(accel_ref = NULL) calls followed by
 // `qd = qd + dt * qdd; q = q + dt * qd`.  The targets are staged once (quaternions normalised as the IK kernels do) or, when
 // none are given, taken from the step-0 walk: p*_l = p_l(q0) and quat*_l = the quaternion of R_l(q0), un-permuted as
-// drmb200_fk_jacobian returns it, so both kinds go through rotvec_error.
+// drmb200_fk_jacobian returns it, so both kinds go through rotvec_error.  DRMB200_IMPLICIT_DAMPING: step 4's ABA takes the
+// pivots d + dt damping (contact_rollout_implicit_kernel), which its unit-response sweeps read back, so qdd_free, G and A
+// are those of the implicit step.
 //
 // Mapping: the contact kernel's (one thread per row, T rows per CTA, the same slot-major row state) with the rollouts' time
 // loop (rollout_pipeline.cuh: state staging, f double buffer, integrate and q / qd / qdd stores).  Once per CTA the
@@ -87,10 +89,12 @@ struct ContactRolloutSmem {
     }
 };
 
-template <int T>
-__global__ void __launch_bounds__(T)
-contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ UnionProgram P,
-                       const __grid_constant__ ContactRolloutArgs args) {
+// The kernel's body, instantiated by contact_rollout_kernel (explicit damping) and contact_rollout_implicit_kernel
+// (IMPLICIT: implicit damping of step h = dt, DRMB200_IMPLICIT_DAMPING): two kernel names rather than a template flag on
+// one, so that the explicit kernel keeps its symbol.
+template <int T, bool IMPLICIT>
+__device__ __forceinline__ void contact_rollout_run(const TreeProgram& prog, const UnionProgram& P,
+                                                    const ContactRolloutArgs& args) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar[2];
 
@@ -173,7 +177,7 @@ contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_co
                 }
             };
             bool ok;
-            DRM_CONTACT_ROW(T, false, true, smem + L.pose + tid, args.flags, args.mu, ok, baumgarte(););
+            DRM_CONTACT_ROW(T, false, true, smem + L.pose + tid, args.flags, args.mu, ok, IMPLICIT, args.dt, baumgarte(););
             solved &= ok ? 1 : 0;
             if (args.qdd != nullptr)
                 for (int c = 0; c < n; ++c) s_qddt[tid * n + c] = smem[L.out + c * T + tid];
@@ -190,6 +194,20 @@ contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_co
     }
     pipe.finish();
     if (tid < valid) args.solved[tile_start + tid] = solved;
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+contact_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ UnionProgram P,
+                       const __grid_constant__ ContactRolloutArgs args) {
+    contact_rollout_run<T, false>(prog, P, args);
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+contact_rollout_implicit_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ UnionProgram P,
+                                const __grid_constant__ ContactRolloutArgs args) {
+    contact_rollout_run<T, true>(prog, P, args);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -209,6 +227,8 @@ int contact_rollout_device(const drmb200_topology_t* topo, int32_t n_ee, const i
         set_error("stabilization=%g: must be finite and >= 0", (double)stabilization);
         return DRMB200_EINVAL;
     }
+    rc = check_implicit_damping(flags, dt);
+    if (rc != DRMB200_OK) return rc;
     if (position_only && target_quat != nullptr) {
         set_error("target_quat must be null for position-only contacts");
         return DRMB200_EINVAL;
@@ -247,6 +267,20 @@ int contact_rollout_device(const drmb200_topology_t* topo, int32_t n_ee, const i
         return DRMB200_ELIMIT;
     }
     const int64_t tiles = (batch + c.tile - 1) / c.tile;
+    if (flags & DRMB200_IMPLICIT_DAMPING) {
+#define DRM_LAUNCH_CONTACT_ROLLOUT(TT) \
+    launch_kernel<contact_rollout_implicit_kernel<TT>>(tiles, TT, c.bytes, stream, false, "contact rollout", *prog, P, args)
+        switch (c.tile) {
+            case 64: return DRM_LAUNCH_CONTACT_ROLLOUT(64);
+            case 32: return DRM_LAUNCH_CONTACT_ROLLOUT(32);
+            case 16: return DRM_LAUNCH_CONTACT_ROLLOUT(16);
+            case 8: return DRM_LAUNCH_CONTACT_ROLLOUT(8);
+            case 4: return DRM_LAUNCH_CONTACT_ROLLOUT(4);
+            case 2: return DRM_LAUNCH_CONTACT_ROLLOUT(2);
+            default: return DRM_LAUNCH_CONTACT_ROLLOUT(1);
+        }
+#undef DRM_LAUNCH_CONTACT_ROLLOUT
+    }
 #define DRM_LAUNCH_CONTACT_ROLLOUT(TT) \
     launch_kernel<contact_rollout_kernel<TT>>(tiles, TT, c.bytes, stream, false, "contact rollout", *prog, P, args)
     switch (c.tile) {

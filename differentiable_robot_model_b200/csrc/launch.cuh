@@ -20,6 +20,17 @@ inline int64_t round256(int64_t bytes) { return (bytes + 255) & ~(int64_t)255; }
 template <typename... P>
 inline bool aligned16(const P*... p) { return (((reinterpret_cast<uintptr_t>(p) & 15u) == 0) && ...); }
 
+// DRMB200_IMPLICIT_DAMPING (include/drm_b200.h) needs DRMB200_DAMPING and a finite step dt > 0; without the flag, OK
+inline int check_implicit_damping(uint32_t flags, float dt) {
+    if (!(flags & DRMB200_IMPLICIT_DAMPING)) return DRMB200_OK;
+    if (!(flags & DRMB200_DAMPING)) { set_error("DRMB200_IMPLICIT_DAMPING needs DRMB200_DAMPING"); return DRMB200_EINVAL; }
+    if (!(dt > 0.f && dt <= 3.40282347e38f)) {                  // NaN and inf fail too
+        set_error("dt=%g: implicit damping needs a finite step > 0", (double)dt);
+        return DRMB200_EINVAL;
+    }
+    return DRMB200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // tile rules: bytes_of(t) is the dynamic shared memory of a CTA of tile t, static_bytes the kernel's static shared memory.
 // A rule returns the tile and its dynamic bytes; the caller refuses the choice (ELIMIT) when bytes + static_bytes exceeds

@@ -9,6 +9,9 @@
 //   qdd_t = FD(q_t, qd_t, tau_t), then the same integrate.  (qd_ref / f absent: 0 - qd_t / 0 + kp e_t; lim absent: no
 //   clamp.)
 // each "+ dt *" one rounded multiply and one rounded add, so that the trajectory is bit-identical to the stepwise torch loop.
+// DRMB200_IMPLICIT_DAMPING: FD is the forward dynamics with implicit damping of step h = dt (rollout_implicit_kernel,
+// pd_rollout_implicit_kernel; aba_body.cuh), and each step of the adjoint runs the implicit ABA adjoint; the integrate and the element-wise step are
+// unchanged.
 //
 // Forward mapping: the articulated-body kernel's (aba.cu) -- one thread per configuration, T per CTA, the same per-thread
 // body (aba_body.cuh) -- with the time loop of rollout_pipeline.cuh inside (rollout_kernel: its own copy).  Once per CTA the table is staged (and folded,
@@ -39,7 +42,7 @@
 namespace drm {
 
 int forward_dynamics_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
-                                     uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t, bool, bool);
+                                     uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t, bool, bool, float);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 
 // u = (f + kp e) + kd ed with e = q_ref - q, ed = qd_ref - qd: the rounding of the torch expression
@@ -89,9 +92,10 @@ struct RolloutSmem {
 // The open-loop kernel keeps its own copy of rollout_pipeline.cuh's time loop: built on RolloutPipeline it compiled to a
 // different schedule of the ABA body (same registers and stack) that measured 1.5-2.5 % slower on an H100 80GB HBM3 at
 // 700 W (DESIGN.md §5), while the PD and contact kernels ran as fast as before.  Its ordering is the pipeline's.
-template <int T>
-__global__ void __launch_bounds__(T)
-rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const RolloutArgs args) {
+// Its body is instantiated by rollout_kernel and rollout_implicit_kernel (IMPLICIT: the forward dynamics with implicit
+// damping of step h = dt, aba_body.cuh), two kernel names rather than a template flag, as for the PD kernel below.
+template <int T, bool IMPLICIT>
+__device__ __forceinline__ void rollout_run(const TreeProgram& prog, const FoldProgram& fold, const RolloutArgs args) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar[2];
 
@@ -152,8 +156,8 @@ rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__
         }
 
         if (tid < valid)
-            aba_body<T>(prog, s_tab, s_q + tid * n, s_qd + tid * n, s_ft + tid * n, s_qddt + tid * n, s_link + tid, s_slot + tid,
-                        args.flags);
+            aba_body<T, IMPLICIT>(prog, s_tab, s_q + tid * n, s_qd + tid * n, s_ft + tid * n, s_qddt + tid * n, s_link + tid,
+                                  s_slot + tid, args.flags, dt);
 
         if (bulk) {
             if (tid == 0) bulk_wait_read<0>();           // the stores of step t - 1 have read s_q / s_qd
@@ -187,6 +191,19 @@ rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__
         }
     }
     if (bulk && tid == 0) bulk_wait_read<0>();
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const RolloutArgs args) {
+    rollout_run<T, false>(prog, fold, args);
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+rollout_implicit_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold,
+                        const RolloutArgs args) {
+    rollout_run<T, true>(prog, fold, args);
 }
 
 struct PDRolloutArgs {
@@ -232,9 +249,10 @@ struct PDRolloutSmem {
     }
 };
 
-template <int T>
-__global__ void __launch_bounds__(T)
-pd_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const PDRolloutArgs args) {
+// The PD kernel's body, instantiated by pd_rollout_kernel (explicit damping) and pd_rollout_implicit_kernel: two kernel
+// names rather than a template flag on one, so that the explicit kernel keeps its symbol.
+template <int T, bool IMPLICIT>
+__device__ __forceinline__ void pd_rollout_run(const TreeProgram& prog, const FoldProgram& fold, const PDRolloutArgs args) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar[2];
 
@@ -284,11 +302,24 @@ pd_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constan
                                            s_kp[gain_row + k], s_kd[gain_row + k], e, ed);
                 taur[k] = has_lim ? pd_clamp(u, s_lim[k]) : u;
             }
-            aba_body<T>(prog, s_tab, qr, qdr, taur, s_qddt + tid * n, s_link + tid, s_slot + tid, args.flags);
+            aba_body<T, IMPLICIT>(prog, s_tab, qr, qdr, taur, s_qddt + tid * n, s_link + tid, s_slot + tid, args.flags, args.dt);
         }
         pipe.integrate_and_store(t, s_qddt + tid * n, 1, args.tau, s_taut, args.qdd, s_qddt);
     }
     pipe.finish();
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+pd_rollout_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold, const PDRolloutArgs args) {
+    pd_rollout_run<T, false>(prog, fold, args);
+}
+
+template <int T>
+__global__ void __launch_bounds__(T)
+pd_rollout_implicit_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold,
+                           const PDRolloutArgs args) {
+    pd_rollout_run<T, true>(prog, fold, args);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -380,11 +411,12 @@ __global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStep
 // host side
 // ---------------------------------------------------------------------------------------------
 // "rnea_fold", as drmb200_forward_dynamics, and the checks both forward rollouts start with
-static int rollout_program(const drmb200_topology_t* topo, int64_t batch, int32_t n_steps, FoldChoice* fc) {
+static int rollout_program(const drmb200_topology_t* topo, int64_t batch, int32_t n_steps, float dt, uint32_t flags,
+                           FoldChoice* fc) {
     const int rc = select_fold(topo, false, fc);
     if (rc != DRMB200_OK) return rc;
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
-    return DRMB200_OK;
+    return check_implicit_damping(flags, dt);
 }
 
 // 64 configurations per CTA when that still gives every SM a CTA and the per-link state leaves room for two CTAs per SM;
@@ -422,7 +454,7 @@ int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float*
                                     const float* f, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q,
                                     float* qd, float* qdd, cudaStream_t stream) {
     FoldChoice fc;
-    const int rc = rollout_program(topo, batch, n_steps, &fc);
+    const int rc = rollout_program(topo, batch, n_steps, dt, flags, &fc);
     if (rc != DRMB200_OK) return rc;
     const TreeProgram& prog = *fc.prog;
     if (batch == 0 || n_steps == 0 || prog.n_dofs == 0) return DRMB200_OK;
@@ -432,9 +464,10 @@ int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float*
     args.table = table; args.q0 = q0; args.qd0 = qd0; args.f = f; args.q = q; args.qd = qd; args.qdd = qdd;
     args.batch = batch; args.n_steps = n_steps; args.dt = dt; args.flags = flags;
     args.aligned = aligned16(q0, qd0, f, q, qd, qdd) && ((batch * prog.n_dofs) & 3) == 0;
-    return launch_rollout<rollout_kernel<64>, rollout_kernel<32>>(fc, batch, [&](int T) {
-        return RolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats;
-    }, "rollout", args, stream);
+    auto floats_of = [&](int T) { return RolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots).total_floats; };
+    if (flags & DRMB200_IMPLICIT_DAMPING)
+        return launch_rollout<rollout_implicit_kernel<64>, rollout_implicit_kernel<32>>(fc, batch, floats_of, "rollout", args, stream);
+    return launch_rollout<rollout_kernel<64>, rollout_kernel<32>>(fc, batch, floats_of, "rollout", args, stream);
 }
 
 int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const float* q0, const float* qd0, const float* q_ref,
@@ -442,7 +475,7 @@ int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const 
                       const float* effort_limit, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q, float* qd,
                       float* qdd, float* tau, cudaStream_t stream) {
     FoldChoice fc;
-    const int rc = rollout_program(topo, batch, n_steps, &fc);
+    const int rc = rollout_program(topo, batch, n_steps, dt, flags, &fc);
     if (rc != DRMB200_OK) return rc;
     const TreeProgram& prog = *fc.prog;
     if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
@@ -460,9 +493,14 @@ int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const 
     args.aligned = aligned16(q0, qd0, q_ref, qd_ref, f, q, qd, qdd, tau) && (!gains_per_row || aligned16(kp, kd)) &&
                    ((batch * prog.n_dofs) & 3) == 0;
     const int n_in = 1 + (qd_ref != nullptr) + (f != nullptr);
-    return launch_rollout<pd_rollout_kernel<64>, pd_rollout_kernel<32>, pd_rollout_kernel<16>>(fc, batch, [&](int T) {
+    auto floats_of = [&](int T) {
         return PDRolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots, n_in, gains_per_row != 0).total_floats;
-    }, "pd rollout", args, stream);
+    };
+    if (flags & DRMB200_IMPLICIT_DAMPING)
+        return launch_rollout<pd_rollout_implicit_kernel<64>, pd_rollout_implicit_kernel<32>, pd_rollout_implicit_kernel<16>>(
+            fc, batch, floats_of, "pd rollout", args, stream);
+    return launch_rollout<pd_rollout_kernel<64>, pd_rollout_kernel<32>, pd_rollout_kernel<16>>(fc, batch, floats_of,
+                                                                                              "pd rollout", args, stream);
 }
 
 // The reverse-time adjoint of both rollouts.  Workspace: [ABA adjoint workspace | a_q | a_qd | g_qdd_t | gq | gqd (| gf
@@ -528,7 +566,7 @@ static int rollout_adjoint(const drmb200_topology_t* topo, const float* table, c
         const float* qdt = t == 0 ? qd0 : qd + (int64_t)(t - 1) * count;
         rc = forward_dynamics_backward_device(topo, table, qt, qdt, tau + (int64_t)t * count, batch, flags, g_step, gq, gqd,
                                               fb ? gf : at(f_grad, t), table_grad, fd_ws, stream,
-                                              /*accumulate_partials=*/t != n_steps - 1, /*reduce=*/t == 0);
+                                              /*accumulate_partials=*/t != n_steps - 1, /*reduce=*/t == 0, dt);
         if (rc != DRMB200_OK) return rc;
     }
     if (!want_final) return DRMB200_OK;
@@ -551,6 +589,7 @@ int forward_dynamics_rollout_backward_device(const drmb200_topology_t* topo, con
                                              float* table_grad, void* workspace, cudaStream_t stream) {
     if (topo == nullptr) { set_error("null topology"); return DRMB200_EINVAL; }
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
+    if (check_implicit_damping(flags, dt) != DRMB200_OK) return DRMB200_EINVAL;
     if (batch == 0 || n_steps == 0 || topo->n_dofs == 0) return DRMB200_OK;
     if (q0_grad == nullptr && qd0_grad == nullptr && f_grad == nullptr && table_grad == nullptr) return DRMB200_OK;
     if (table == nullptr || q0 == nullptr || qd0 == nullptr || f == nullptr || (n_steps > 1 && (q == nullptr || qd == nullptr))) {
@@ -575,6 +614,7 @@ int pd_rollout_backward_device(const drmb200_topology_t* topo, const float* tabl
                                float* table_grad, void* workspace, cudaStream_t stream) {
     if (topo == nullptr) { set_error("null topology"); return DRMB200_EINVAL; }
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
+    if (check_implicit_damping(flags, dt) != DRMB200_OK) return DRMB200_EINVAL;
     if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
     if (batch == 0 || n_steps == 0 || topo->n_dofs == 0) return DRMB200_OK;
     const bool want_elementwise = q0_grad || qd0_grad || q_ref_grad || qd_ref_grad || f_grad || kp_grad || kd_grad;

@@ -23,6 +23,7 @@ _lib = None
 GRAVITY = 1
 DAMPING = 2
 INERTIAL_GRADS_ONLY = 4      # backward hint: no kinematic link parameter is learnable (see include/drm_b200.h)
+IMPLICIT_DAMPING = 8         # rollouts: the damping torque taken at the end-of-step velocity (see include/drm_b200.h)
 
 _c_float_p = ctypes.c_void_p      # raw device / host addresses
 _SIGNATURES = {
@@ -69,6 +70,14 @@ _SIGNATURES = {
                                                          _c_float_p, ctypes.c_int64, ctypes.c_uint32, _c_float_p,
                                                          _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                          ctypes.c_void_p, ctypes.c_void_p]),
+    "drmb200_forward_dynamics_implicit_damping": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p,
+                                                                 _c_float_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_float,
+                                                                 _c_float_p, ctypes.c_void_p]),
+    "drmb200_forward_dynamics_implicit_damping_backward": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p,
+                                                                          _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_uint32,
+                                                                          ctypes.c_float, _c_float_p, _c_float_p, _c_float_p,
+                                                                          _c_float_p, _c_float_p, ctypes.c_void_p,
+                                                                          ctypes.c_void_p]),
     "drmb200_forward_dynamics_rollout": (ctypes.c_int, [ctypes.POINTER(Topology), _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                                         ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_uint32,
                                                         _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
@@ -334,13 +343,19 @@ def inverse_dynamics_raw(topo, table, q, qd, qdd, flags, out=None, folded=None):
     return tau
 
 
-def forward_dynamics_raw(topo, table, q, qd, f, flags, out=None, folded=None):
-    """Articulated-body algorithm, one launch (drmb200_forward_dynamics; `folded`: rows of fold_link_table for an unchanged table)."""
+def forward_dynamics_raw(topo, table, q, qd, f, flags, out=None, folded=None, implicit_dt=None):
+    """Articulated-body algorithm, one launch (drmb200_forward_dynamics; `folded`: rows of fold_link_table for an unchanged table).
+    implicit_dt: implicit damping with that step (drmb200_forward_dynamics_implicit_damping, on the unfolded table)."""
     _require_cuda(table, q, qd, f, folded)
     q, qd, f = q.contiguous(), qd.contiguous(), f.contiguous()
     B, n = q.shape
     qdd = out if out is not None else torch.empty((B, n), device=q.device, dtype=torch.float32)
     with _on(q.device):
+        if implicit_dt is not None:
+            rc = lib().drmb200_forward_dynamics_implicit_damping(ctypes.byref(topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B,
+                                                                 flags, ctypes.c_float(implicit_dt), _ptr(qdd), _stream())
+            _check(rc, "drmb200_forward_dynamics_implicit_damping")
+            return qdd
         if folded is not None:
             rc = lib().drmb200_forward_dynamics_prefolded(ctypes.byref(topo), _ptr(folded), _ptr(q), _ptr(qd), _ptr(f), B,
                                                           flags, _ptr(qdd), _stream())
@@ -688,7 +703,8 @@ def contact_rollout_raw(topo, ee_links, table, q0, qd0, f, dt, flags, target_pos
     links = (ctypes.c_int32 * max(E, 1))(*[int(l) for l in ee_links])
     with _on(dev):
         rc = lib().drmb200_contact_rollout(ctypes.byref(topo), E, links, _ptr(table), _ptr(q0), _ptr(qd0), _ptr(f),
-                                           _ptr(target_pos), _ptr(target_quat), B, T, ctypes.c_float(dt), flags & 3,
+                                           _ptr(target_pos), _ptr(target_quat), B, T, ctypes.c_float(dt),
+                                           flags & (GRAVITY | DAMPING | IMPLICIT_DAMPING),
                                            1 if position_only else 0, ctypes.c_float(regularization),
                                            ctypes.c_float(stabilization), _ptr(q), _ptr(qd), _ptr(qdd), _ptr(force),
                                            _ptr(accel_ref), _ptr(solved), _stream())
@@ -1010,14 +1026,15 @@ class InverseDynamicsFunction(torch.autograd.Function):
 
 
 class ForwardDynamicsFunction(torch.autograd.Function):
-    """(table, q, qd, f) -> qdd; articulated-body kernel forward, analytic adjoint kernel backward."""
+    """(table, q, qd, f) -> qdd; articulated-body kernel forward, analytic adjoint kernel backward.  implicit_dt: implicit
+    damping with that step (not differentiated)."""
 
     @staticmethod
-    def forward(ctx, table, q, qd, f, topo, flags, folded=None):
+    def forward(ctx, table, q, qd, f, topo, flags, folded=None, implicit_dt=None):
         ctx.save_for_backward(table, q, qd, f)  # as given, not the contiguous copies: first_order_only links to them
         table, q, qd, f = table.contiguous(), q.contiguous(), qd.contiguous(), f.contiguous()
-        qdd = forward_dynamics_raw(topo, table, q, qd, f, flags, folded=folded)
-        ctx.topo, ctx.flags = topo, flags
+        qdd = forward_dynamics_raw(topo, table, q, qd, f, flags, folded=folded, implicit_dt=implicit_dt)
+        ctx.topo, ctx.flags, ctx.implicit_dt = topo, flags, implicit_dt
         return qdd
 
     @staticmethod
@@ -1035,11 +1052,17 @@ class ForwardDynamicsFunction(torch.autograd.Function):
         nbytes = int(lib().drmb200_forward_dynamics_backward_workspace_bytes(ctypes.byref(ctx.topo), B))
         ws = torch.empty((nbytes + 3) // 4, device=q.device, dtype=torch.float32)
         with _on(q.device):
-            rc = lib().drmb200_forward_dynamics_backward(
-                ctypes.byref(ctx.topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B, ctx.flags, _ptr(g_qdd), _ptr(q_grad), _ptr(qd_grad),
-                _ptr(f_grad), _ptr(table_grad), _ptr(ws), _stream())
-        _check(rc, "drmb200_forward_dynamics_backward")
-        return first_order_only((table_grad, q_grad, qd_grad, f_grad), saved + (g_qdd,)) + (None,) * 3
+            if ctx.implicit_dt is not None:
+                rc = lib().drmb200_forward_dynamics_implicit_damping_backward(
+                    ctypes.byref(ctx.topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B, ctx.flags, ctypes.c_float(ctx.implicit_dt),
+                    _ptr(g_qdd), _ptr(q_grad), _ptr(qd_grad), _ptr(f_grad), _ptr(table_grad), _ptr(ws), _stream())
+                _check(rc, "drmb200_forward_dynamics_implicit_damping_backward")
+            else:
+                rc = lib().drmb200_forward_dynamics_backward(
+                    ctypes.byref(ctx.topo), _ptr(table), _ptr(q), _ptr(qd), _ptr(f), B, ctx.flags, _ptr(g_qdd), _ptr(q_grad), _ptr(qd_grad),
+                    _ptr(f_grad), _ptr(table_grad), _ptr(ws), _stream())
+                _check(rc, "drmb200_forward_dynamics_backward")
+        return first_order_only((table_grad, q_grad, qd_grad, f_grad), saved + (g_qdd,)) + (None,) * 4
 
 
 class ForwardDynamicsRolloutFunction(torch.autograd.Function):

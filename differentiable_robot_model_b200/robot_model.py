@@ -481,14 +481,25 @@ class DifferentiableRobotModel(torch.nn.Module):
         f: torch.Tensor,
         include_gravity: Optional[bool] = True,
         use_damping: Optional[bool] = False,
+        implicit_damping_dt: Optional[float] = None,
     ) -> torch.Tensor:
         r"""Joint accelerations under applied joint forces ``f``: the articulated-body algorithm of
         ``robot_model.py:488-624`` in ONE launch (``csrc/aba.cu``), with the reference's arithmetic (general 6x6
         articulated inertias -- ``inertia_mat`` is never symmetrised --, ``+1e-37`` regularisers).  Differentiable
         w.r.t. q, qd, f and every learnable link parameter through the analytic adjoint kernel.  Unlike the reference
-        this does not overwrite the caller's ``f`` when ``use_damping`` is set (``robot_model.py:521``)."""
+        this does not overwrite the caller's ``f`` when ``use_damping`` is set (``robot_model.py:521``).
+
+        ``implicit_damping_dt = h`` (needs ``use_damping``) treats the joint damping implicitly for a step of length ``h``:
+        every joint's articulated-body pivot ``d`` becomes ``d + h * damping``, which for symmetric inertias gives
+        ``(H + h diag(damping))^-1 (f - nle(q, qd))``, the acceleration of a semi-implicit Euler step whose damping torque
+        is taken at the end-of-step velocity ``qd + h qdd``.  Such a step is stable at any ``h``, however strongly damped
+        and light the links (``include/drm_b200.h``: ``drmb200_forward_dynamics_implicit_damping``).  ``h`` is not
+        differentiated."""
         self._check_q(q, qd, f)
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        if implicit_damping_dt is not None:
+            h = self._implicit_damping_step(True, use_damping, implicit_damping_dt)
+            return engine.ForwardDynamicsFunction.apply(self._link_table(), q, qd, f, self._topology, flags, None, h)
         return engine.ForwardDynamicsFunction.apply(self._link_table(), q, qd, f, self._topology, flags, self._folded_table())
 
     @tensor_check
@@ -920,6 +931,16 @@ class DifferentiableRobotModel(torch.nn.Module):
         return q0.ndim == 1
 
     @staticmethod
+    def _implicit_damping_step(implicit, use_damping, dt):
+        """The checks of ``implicit_damping`` / ``implicit_damping_dt``: ``use_damping`` is set and the step ``dt`` is finite
+        and > 0.  Returns ``float(dt)``."""
+        dt = float(dt)
+        if implicit:
+            assert use_damping, "implicit damping needs use_damping=True"
+            assert 0.0 < dt < float("inf"), f"implicit damping needs a finite step dt > 0 (got {dt})"
+        return dt
+
+    @staticmethod
     def _rollout_batch_dim(q0, qd0, *per_step):
         """1-D rollout inputs with the batch dimension of one row added: ``q0`` / ``qd0`` in front, every per-step (or
         per-link) tensor after its leading dimension; None stays None."""
@@ -933,6 +954,7 @@ class DifferentiableRobotModel(torch.nn.Module):
         dt: float,
         include_gravity: Optional[bool] = True,
         use_damping: Optional[bool] = False,
+        implicit_damping: bool = False,
     ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         r"""Integrate :meth:`compute_forward_dynamics` over ``T`` steps of semi-implicit (symplectic) Euler in ONE launch
         (``csrc/rollout.cu``).  From ``(q_0, qd_0) = (q0, qd0)``, step ``t`` computes in fp32, in this order::
@@ -941,7 +963,10 @@ class DifferentiableRobotModel(torch.nn.Module):
             qd_{t+1} = qd_t + dt * qdd_t
             q_{t+1} = q_t + dt * qd_{t+1}
 
-        and the result is bit-identical to that Python loop on the same model.
+        and the result is bit-identical to that Python loop on the same model.  With ``implicit_damping`` (which needs
+        ``use_damping``) step t calls ``compute_forward_dynamics(..., implicit_damping_dt=dt)`` instead: the damping torque
+        is taken at the end-of-step velocity, so strongly damped light links (the Allegro fingers) stay stable at any ``dt``,
+        where the explicit damping diverges above about ``dt = 2 I / d``.
 
         Args:
             q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
@@ -954,8 +979,9 @@ class DifferentiableRobotModel(torch.nn.Module):
         if squeeze:
             q0, qd0, f = self._rollout_batch_dim(q0, qd0, f)
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        flags |= engine.IMPLICIT_DAMPING if implicit_damping else 0
         table = self._link_table()
-        dt = float(dt)
+        dt = self._implicit_damping_step(implicit_damping, use_damping, dt)
         if torch.is_grad_enabled() and (table.requires_grad or q0.requires_grad or qd0.requires_grad or f.requires_grad):
             out = engine.ForwardDynamicsRolloutFunction.apply(table, q0, qd0, f, self._topology, flags, dt)
         else:
@@ -976,6 +1002,7 @@ class DifferentiableRobotModel(torch.nn.Module):
         use_damping: Optional[bool] = False,
         position_only: bool = False,
         regularization: float = 0.0,
+        implicit_damping: bool = False,
     ) -> ContactRollout:
         r"""Simulate the links held by bilateral rigid contacts: :meth:`compute_contact_dynamics` integrated over ``T`` steps
         of semi-implicit Euler, with Baumgarte stabilisation towards fixed targets, all in ONE launch
@@ -994,7 +1021,9 @@ class DifferentiableRobotModel(torch.nn.Module):
         With ``use_damping`` the joints' damping torque ``-d qd`` enters each step at the current ``qd``, so the integrate is
         explicit in it and stable only for ``dt`` below about ``2 I / d`` (``I`` a joint's effective inertia): the Allegro
         hand's fingers (damping 3-8 N m s/rad on links of a few grams) diverge within ten steps at ``dt = 1e-3`` and at
-        ``1e-4``; simulate them without damping or at a far smaller step.
+        ``1e-4``.  Simulate them with ``implicit_damping=True``: every step's forward dynamics and force response then
+        take the damping implicitly (``compute_forward_dynamics(..., implicit_damping_dt=dt)``), which is stable at any
+        ``dt``.
 
         Args:
             q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
@@ -1008,6 +1037,7 @@ class DifferentiableRobotModel(torch.nn.Module):
                 given together with ``target_pos``; must be None with ``position_only``
             stabilization: the Baumgarte rate ``w >= 0`` [1/s]
             include_gravity, use_damping, position_only, regularization: as for :meth:`compute_contact_dynamics`
+            implicit_damping: take the damping implicitly with step ``dt`` (needs ``use_damping``)
         Returns: :class:`ContactRollout` ``(q, qd, qdd, force, solved)`` with ``q[t] = q_{t+1}``, ``qd[t] = qd_{t+1}``,
         ``qdd[t] = qdd_t`` and ``force[t]`` the contact forces of step ``t``; the batch dimension is dropped for 1-D inputs.
         ``solved`` is False for a row where some step was not solved; that step and every later one of the row are NaN.
@@ -1029,8 +1059,10 @@ class DifferentiableRobotModel(torch.nn.Module):
         assert target_pos is None or tuple(target_pos.shape) == (E, B, 3), "target_pos must be [n_links x batch_size x 3]"
         assert target_quat is None or tuple(target_quat.shape) == (E, B, 4), "target_quat must be [n_links x batch_size x 4]"
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        flags |= engine.IMPLICIT_DAMPING if implicit_damping else 0
+        dt = self._implicit_damping_step(implicit_damping, use_damping, dt)
         q, qd, qdd, force, _, solved = engine.contact_rollout_raw(
-            self._topology, links, self._link_table().detach(), q0.detach(), qd0.detach(), f.detach(), float(dt), flags,
+            self._topology, links, self._link_table().detach(), q0.detach(), qd0.detach(), f.detach(), dt, flags,
             None if target_pos is None else target_pos.detach(), None if target_quat is None else target_quat.detach(),
             bool(position_only), float(regularization), stabilization)
         if squeeze:
@@ -1050,6 +1082,7 @@ class DifferentiableRobotModel(torch.nn.Module):
         effort_limit: Optional[torch.Tensor] = None,
         include_gravity: Optional[bool] = True,
         use_damping: Optional[bool] = False,
+        implicit_damping: bool = False,
     ) -> ControlledRollout:
         r"""Simulate a joint-space PD controller tracking reference trajectories: :meth:`compute_forward_dynamics_rollout`
         with the torque of every step computed from the current state, all ``T`` steps in ONE launch
@@ -1061,7 +1094,9 @@ class DifferentiableRobotModel(torch.nn.Module):
             qd = qd + dt * qdd
             q = q + dt * qd
 
-        and the result is bit-identical to that Python loop on the same model.
+        and the result is bit-identical to that Python loop on the same model; with ``implicit_damping`` (needs
+        ``use_damping``) the loop's call is ``compute_forward_dynamics(q, qd, u, ..., implicit_damping_dt=dt)``, stable in
+        the joint damping at any ``dt``.
 
         Args:
             q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
@@ -1098,8 +1133,9 @@ class DifferentiableRobotModel(torch.nn.Module):
         if squeeze:
             q0, qd0, q_ref, qd_ref, f = self._rollout_batch_dim(q0, qd0, q_ref, qd_ref, f)
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
+        flags |= engine.IMPLICIT_DAMPING if implicit_damping else 0
         table = self._link_table()
-        dt = float(dt)
+        dt = self._implicit_damping_step(implicit_damping, use_damping, dt)
         lim = None if effort_limit is None else effort_limit.detach()
         if kp.shape != kd.shape:
             # the kernel reads both gains in one layout: the shared one becomes a per-row view (its gradient is the sum of

@@ -89,6 +89,10 @@ extern "C" {
  * and the damping column -- nothing kinematic (F, r) is learnable and q_grad / qd_grad / qdd_grad are NULL.
  * Selects a single-sweep kernel (~6x fewer instructions); the F / r columns of table_grad are left untouched. */
 #define DRMB200_INERTIAL_GRADS_ONLY 4u
+/* the rollouts (drmb200_forward_dynamics_rollout(_backward), drmb200_pd_rollout(_backward), drmb200_contact_rollout) only:
+ * implicit joint damping with step h = dt, as defined at drmb200_forward_dynamics_implicit_damping.  Needs
+ * DRMB200_DAMPING and a finite dt > 0, else DRMB200_EINVAL. */
+#define DRMB200_IMPLICIT_DAMPING 8u
 
 /*
  * Immutable kinematic-tree topology, host memory, links in URDF document order
@@ -258,11 +262,37 @@ int drmb200_forward_dynamics_backward(const drmb200_topology_t* topo,
                                       float* table_grad, void* workspace, void* cuda_stream);
 
 /*
+ * Forward dynamics with implicit joint damping of step h = dt > 0 (finite): the articulated-body arithmetic of
+ * drmb200_forward_dynamics with one change -- every movable joint's pivot d_i = S^T IA_i S becomes d_i + h damping_i
+ * wherever it is used (the 1/(d + 1e-37) of the articulated-inertia pass, the 1/d of the acceleration pass).  The damping
+ * torque -damping * qd is still applied, so flags must hold DRMB200_DAMPING (DRMB200_GRAVITY as for
+ * drmb200_forward_dynamics; DRMB200_IMPLICIT_DAMPING is implied).  For a symmetric inertia this is
+ *     qdd = (H(q) + h diag(damping))^-1 (f - nle(q, qd)),   nle including the damping torque,
+ * the acceleration of a semi-implicit Euler step of length h whose damping torque is taken at the end-of-step velocity
+ * qd + h qdd: the step is unconditionally stable in the damping, where the explicit one needs h below about 2 I / d.  For a
+ * non-symmetric inertia_mat the arithmetic is the definition, as for drmb200_forward_dynamics.  The rollouts take exactly
+ * this qdd_t (h = dt) with DRMB200_IMPLICIT_DAMPING.  The backward is the analytic adjoint of that arithmetic: the pivot's
+ * adjoint also reaches the damping column of table_grad; dt is not differentiated.  Its workspace is
+ * drmb200_forward_dynamics_backward_workspace_bytes().  DRMB200_EINVAL without DRMB200_DAMPING or for a dt that is not
+ * finite and > 0; otherwise the errors of drmb200_forward_dynamics / drmb200_forward_dynamics_backward.
+ */
+int drmb200_forward_dynamics_implicit_damping(const drmb200_topology_t* topo,
+                                              const float* table, const float* q, const float* qd, const float* f,
+                                              int64_t batch, uint32_t flags, float dt, float* qdd, void* cuda_stream);
+int drmb200_forward_dynamics_implicit_damping_backward(const drmb200_topology_t* topo,
+                                                       const float* table, const float* q, const float* qd, const float* f,
+                                                       int64_t batch, uint32_t flags, float dt, const float* g_qdd,
+                                                       float* q_grad, float* qd_grad, float* f_grad,
+                                                       float* table_grad, void* workspace, void* cuda_stream);
+
+/*
  * Forward-dynamics rollout: n_steps steps of semi-implicit (symplectic) Euler over drmb200_forward_dynamics in ONE launch.
  * Starting from (q_0, qd_0) = (q0, qd0), step t = 0 .. n_steps-1 computes, in fp32 and in exactly this order,
  *     qdd_t = FD(q_t, qd_t, f_t);   qd_{t+1} = qd_t + dt * qdd_t;   q_{t+1} = q_t + dt * qd_{t+1}
  * (each "+ dt *" a rounded multiply, then a rounded add -- no FMA), so the trajectory is bit-identical to a loop of
- * drmb200_forward_dynamics launches followed by those two updates.  flags mean what they mean for drmb200_forward_dynamics.
+ * drmb200_forward_dynamics launches followed by those two updates.  flags mean what they mean for drmb200_forward_dynamics;
+ * with DRMB200_IMPLICIT_DAMPING (and DRMB200_DAMPING) FD is drmb200_forward_dynamics_implicit_damping with h = dt, and the
+ * trajectory is bit-identical to a loop of those launches.
  * Layout is time-major:
  *   q0, qd0              [B, n_dofs]
  *   f                    [n_steps, B, n_dofs]   applied joint forces of every step (never modified)
@@ -282,7 +312,8 @@ int drmb200_forward_dynamics_rollout(const drmb200_topology_t* topo, const float
  * into table_grad (may be NULL).  Runs the analytic adjoint of drmb200_forward_dynamics_backward once per step, t = n_steps-1
  * .. 0, with one element-wise launch per step between them (2 n_steps + 2 launches).  `workspace` must hold
  * drmb200_forward_dynamics_rollout_backward_workspace_bytes(topo, batch) bytes; it does not depend on n_steps.  Outputs
- * must not alias inputs.
+ * must not alias inputs.  With DRMB200_IMPLICIT_DAMPING each step runs the adjoint of
+ * drmb200_forward_dynamics_implicit_damping_backward (h = dt).
  */
 int64_t drmb200_forward_dynamics_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch);
 int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, const float* table,
@@ -303,6 +334,8 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
  *                                                       multiply, then a rounded add
  *     tau_t = clamp(u_t, -effort_limit, effort_limit)   only when effort_limit is given; NaN propagates (torch.clamp)
  *     qdd_t = FD(q_t, qd_t, tau_t)                      exactly drmb200_forward_dynamics with the same flags
+ *                                                       (drmb200_forward_dynamics_implicit_damping with h = dt under
+ *                                                       DRMB200_IMPLICIT_DAMPING)
  *     qd_{t+1} = qd_t + dt * qdd_t;   q_{t+1} = q_t + dt * qd_{t+1}   as drmb200_forward_dynamics_rollout
  * so the trajectory is bit-identical to the torch loop
  *     u = f[t] + kp * (q_ref[t] - q) + kd * (qd_ref[t] - qd); u = clamp(u, -lim, lim);
@@ -334,8 +367,8 @@ int drmb200_pd_rollout(const drmb200_topology_t* topo, const float* table,
  * gradient is their sum over rows); each may be NULL.  Accumulates the table gradient of all steps into table_grad (may be
  * NULL).  The clamp passes the gradient where -effort_limit <= u_t <= effort_limit (torch.clamp's rule), u_t recomputed
  * bit-exactly.  Runs the analytic adjoint of drmb200_forward_dynamics_backward once per step, t = n_steps-1 .. 0, at
- * (q_t, qd_t, tau_t), with one element-wise launch per step between them (2 n_steps + 2 launches, no atomics: bitwise
- * reproducible).  `workspace` must hold drmb200_pd_rollout_backward_workspace_bytes(topo, batch) bytes; it does not depend
+ * (q_t, qd_t, tau_t) (the implicit-damping adjoint under DRMB200_IMPLICIT_DAMPING), with one element-wise launch per
+ * step between them (2 n_steps + 2 launches, no atomics: bitwise reproducible).  `workspace` must hold drmb200_pd_rollout_backward_workspace_bytes(topo, batch) bytes; it does not depend
  * on n_steps.  Outputs must not alias inputs.
  */
 int64_t drmb200_pd_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch);
@@ -583,7 +616,10 @@ int drmb200_contact_impulse_backward(const drmb200_topology_t* topo, int32_t n_e
  *   5. qd_{t+1} = qd_t + dt * qdd_t;  q_{t+1} = q_t + dt * qd_{t+1}, every product and sum rounded separately.
  * With DRMB200_DAMPING the damping torque -d qd_t enters qdd_t explicitly, so the integrate is stable only for dt below
  * about 2 I / d (I a joint's effective inertia); light, strongly damped links need a far smaller step (the Allegro
- * fingers diverge within ten steps at dt = 1 ms and at 0.1 ms).
+ * fingers diverge within ten steps at dt = 1 ms and at 0.1 ms).  DRMB200_IMPLICIT_DAMPING (with DRMB200_DAMPING) takes
+ * the damping implicitly: G and qdd_free become those of drmb200_forward_dynamics_implicit_damping with h = dt (pivots
+ * d + dt damping in the ABA and in every unit-response sweep), so A = J G J^T + mu I follows; the step is stable in the
+ * damping at any dt.
  * Outputs, time-major, caller-allocated, must not alias inputs: q [T, B, n] (q[t] = q_{t+1}), qd [T, B, n], qdd [T, B, n]
  * (qdd_t) or NULL, force [T, B, M] (lambda_t) or NULL, accel_ref [T, B, M] (the a_ref of step t) or NULL, solved [B] uint8
  * (the AND of ok_t over all steps).  An unsolved step gives NaN in qdd and lambda, so the row's state is NaN from then on;
