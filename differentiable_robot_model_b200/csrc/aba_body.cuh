@@ -145,10 +145,13 @@ __device__ __forceinline__ void sub_outer_pp(M3PP& m, V3 x, const V3P& yp) {
 // IMPLICIT: implicit joint damping with step h (include/drm_b200.h) -- every movable joint's pivot d = S^T IA S becomes
 // d + h damping wherever it is used (passes 2 and 3 here, and the unit-response sweeps that read the stored d), which gives
 // (H + h diag(damping))^-1 (f - nle) for symmetric inertias.  The damping torque itself still needs DRMB200_DAMPING.
-template <int T, bool IMPLICIT = false>
+// ADDEND: a per-row pivot addend -- every movable joint's pivot (after the implicit damping's term) then gets + crow[dof]
+// in one rounded add, read back by pass 3 like the rest of the pivot: (H (+ h D) + diag(crow))^-1 (f - nle) for symmetric
+// inertias, the implicit PD gains of the PD rollout (rollout.cu, DRMB200_IMPLICIT_GAINS).
+template <int T, bool IMPLICIT = false, bool ADDEND = false>
 __device__ __forceinline__ void aba_body(const TreeProgram& prog, const float* s_tab, const float* qrow, const float* qdrow,
                                          const float* frow, float* outrow, float* lk0, float* sl0, uint32_t flags,
-                                         float h = 0.f) {
+                                         float h = 0.f, const float* crow = nullptr) {
     const int N = prog.n_links;
     const float g = (flags & DRMB200_GRAVITY) ? ABA_GRAVITY : 0.f;
     const bool damp = (flags & DRMB200_DAMPING) != 0;
@@ -221,6 +224,7 @@ __device__ __forceinline__ void aba_body(const TreeProgram& prog, const float* s
                 upk2(CD.a02, Ul.x, t); upk2(CD.a12, Ul.y, t); upk2(CD.a22, Ul.z, t);
                 d = Ua.z;                                                      // S . U                    (:557)
                 if constexpr (IMPLICIT) d = fmaf(h, C.d, d);                   // + h damping
+                if constexpr (ADDEND) d = __fadd_rn(d, crow[c]);               // + the row's addend
                 float fk = frow[c];
                 if (damp) fk = fmaf(-C.d, qdrow[c], fk);                       // f -= damping * qd        (:516-521)
                 u = fk - p_ang.z;                                              // (:559)

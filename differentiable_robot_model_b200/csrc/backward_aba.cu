@@ -46,6 +46,9 @@ struct AbaBwdArgs {
     int32_t vec_ok;
     int32_t accumulate;                // add to the per-CTA partial tables instead of overwriting them
     float h;                           // IMPLICIT: the step of the implicit damping
+    const float* __restrict__ c;       // ADDEND: the per-row pivot addends [B, n]
+    float* __restrict__ c_grad;        // ADDEND: their adjoints, the pivots' d-bar [B, n]
+    float* __restrict__ qdd;           // ADDEND: the recomputed accelerations [B, n]
 };
 
 struct AbaBwdSmem {
@@ -148,9 +151,11 @@ __device__ __forceinline__ void st_blocks(float* p, int T, const Blocks& b) {
 
 // IMPLICIT: the adjoint of aba_body<T, true> -- every use of Ua.z as the pivot becomes Ua.z + h damping, and the pivot's
 // adjoint d-bar also reaches the damping column of the table (h d-bar, on top of the damping torque's -u-bar qd).
-template <bool NEED_TABLE, int T, bool IMPLICIT = false>
-__global__ void __launch_bounds__(T < 32 ? 32 : T)
-aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs args) {
+// ADDEND: the adjoint of aba_body<T, IMPLICIT, true> -- the pivot then gets + c[row, dof] (args.c); the pivot's d-bar is
+// c's adjoint (args.c_grad), and F3's accelerations go to args.qdd.  The body is instantiated by aba_backward_kernel and
+// aba_backward_addend_kernel, so that the kernel without the addend keeps its symbol.
+template <bool NEED_TABLE, int T, bool IMPLICIT, bool ADDEND>
+__device__ __forceinline__ void aba_backward_run(const TreeProgram& prog, const AbaBwdArgs args) {
     constexpr int TB = T < 32 ? 32 : T;
     static_assert(TB == 32, "warp_accumulate assumes a single-warp CTA");
     extern __shared__ __align__(128) float smem[];
@@ -171,7 +176,12 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
     const bool vec_ok = args.vec_ok;
     const float grav = (args.flags & DRMB200_GRAVITY) ? GRAVITY_B : 0.f;
     const bool damp = (args.flags & DRMB200_DAMPING) != 0;
-    auto pivot = [&](float uz, int i) { return IMPLICIT ? fmaf(args.h, s_tab[i * DRMB200_TABLE_STRIDE + 25], uz) : uz; };
+    const float* crow = nullptr;                        // ADDEND: this thread's row of c
+    auto pivot = [&](float uz, int i) {
+        const float d = IMPLICIT ? fmaf(args.h, s_tab[i * DRMB200_TABLE_STRIDE + 25], uz) : uz;
+        if constexpr (ADDEND) return __fadd_rn(d, crow[prog.dof[i]]);
+        else return d;
+    };
 
     for (int i = tid; i < N * DRMB200_TABLE_STRIDE; i += TB) {
         const int l = i / DRMB200_TABLE_STRIDE, e = i - l * DRMB200_TABLE_STRIDE;
@@ -207,6 +217,8 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
         float* gia0 = args.scratch + ((int64_t)blockIdx.x * (N - 1) - 1) * IA_FLOATS * T + lane;     // IA of link i at gia0 + i * 36 * T
         const V3 zero = v3(0.f, 0.f, 0.f);
         const bool writer = tid < T;                    // shadows must not store
+        const int64_t grow_off = (start + (active ? lane : 0)) * n;     // ADDEND: rows past the batch read row 0's c
+        if constexpr (ADDEND) crow = args.c + grow_off;
 
         // ================= F1: velocities, bias forces, rigid-body inertias =====================
         for (int i = 1; i < N; ++i) {
@@ -306,6 +318,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
                 const V3 Ua = v3(gia0[(i * IA_FLOATS + 2) * T], gia0[(i * IA_FLOATS + 5) * T], gia0[(i * IA_FLOATS + 8) * T]);
                 const V3 Ul = v3(gia0[(i * IA_FLOATS + 20) * T], gia0[(i * IA_FLOATS + 23) * T], gia0[(i * IA_FLOATS + 26) * T]);
                 const float qdd = (1.0f / pivot(Ua.z, i)) * (lk[O_U * T] - (dot(Ua, al) + dot(Ul, a)));
+                if constexpr (ADDEND) { if (active) args.qdd[grow_off + c] = qdd; }
                 al.z += qdd;
             }
             if (writer) { stv(lk + O_AL * T, T, al); stv(lk + (O_AL + 3) * T, T, a); }
@@ -468,6 +481,7 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
             }
             if (c >= 0) {
                 if (writer) fg[c] = ub;
+                if constexpr (ADDEND) { if (active) args.c_grad[grow_off + c] = db; }      // d-bar is final here
                 if (damp) {
                     if (writer) qdg[c] = fmaf(-s_tab[i * DRMB200_TABLE_STRIDE + 25], ub, qdg[c]);
                     vals[25] = -ub * qdrow[c];
@@ -565,6 +579,18 @@ aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs a
     }
 }
 
+template <bool NEED_TABLE, int T, bool IMPLICIT = false>
+__global__ void __launch_bounds__(T < 32 ? 32 : T)
+aba_backward_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs args) {
+    aba_backward_run<NEED_TABLE, T, IMPLICIT, false>(prog, args);
+}
+
+template <bool NEED_TABLE, int T, bool IMPLICIT>
+__global__ void __launch_bounds__(T < 32 ? 32 : T)
+aba_backward_addend_kernel(const __grid_constant__ TreeProgram prog, const AbaBwdArgs args) {
+    aba_backward_run<NEED_TABLE, T, IMPLICIT, true>(prog, args);
+}
+
 // workspace = per-CTA partial tables (as for the other backward kernels) + the per-CTA articulated-inertia scratch
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch) {
     if (topo == nullptr || topo->n_links < 1 || topo->n_links > DRMB200_MAX_LINKS) return 0;
@@ -577,18 +603,25 @@ int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t* topo
 // accumulate_partials / reduce: a caller that runs the adjoint several times on batches of the same size (the steps of a
 // rollout, rollout.cu) can sum the per-CTA partial tables of all calls in the workspace and reduce them into table_grad once,
 // with the last call; the default (false, true) is one self-contained adjoint.  With DRMB200_IMPLICIT_DAMPING in flags,
-// the adjoint of the forward dynamics with implicit damping of step dt (checked by the caller).
+// the adjoint of the forward dynamics with implicit damping of step dt (checked by the caller).  c != NULL: the adjoint of
+// the forward dynamics whose pivots get the per-row addends c [B, n] (aba_body's ADDEND, the PD rollout's implicit gains);
+// it writes their adjoints to c_grad and the recomputed accelerations to qdd_out, both [B, n] and required then.
 int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
                                      const float* f, int64_t batch, uint32_t flags, const float* g_qdd,
                                      float* q_grad, float* qd_grad, float* f_grad, float* table_grad, void* workspace,
-                                     cudaStream_t stream, bool accumulate_partials, bool reduce, float dt) {
+                                     cudaStream_t stream, bool accumulate_partials, bool reduce, float dt,
+                                     const float* c, float* c_grad, float* qdd_out) {
     TreeProgram prog;
     int rc = build_tree_program(topo, &prog);
     if (rc != DRMB200_OK) return rc;
     if (batch < 0) { set_error("batch=%lld < 0", (long long)batch); return DRMB200_EINVAL; }
     if (batch == 0 || prog.n_dofs == 0) return DRMB200_OK;
-    if (q_grad == nullptr && qd_grad == nullptr && f_grad == nullptr && table_grad == nullptr) return DRMB200_OK;
-    if (table == nullptr || q == nullptr || qd == nullptr || f == nullptr || g_qdd == nullptr) { set_error("null pointer argument"); return DRMB200_EINVAL; }
+    if (q_grad == nullptr && qd_grad == nullptr && f_grad == nullptr && table_grad == nullptr && c == nullptr) return DRMB200_OK;
+    if (table == nullptr || q == nullptr || qd == nullptr || f == nullptr || g_qdd == nullptr ||
+        (c != nullptr && (c_grad == nullptr || qdd_out == nullptr))) {
+        set_error("null pointer argument");
+        return DRMB200_EINVAL;
+    }
     if (workspace == nullptr) { set_error("forward-dynamics backward needs its workspace (drmb200_forward_dynamics_backward_workspace_bytes)"); return DRMB200_EINVAL; }
 
     AbaBwdArgs args;
@@ -599,6 +632,7 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     args.batch = batch; args.flags = flags;
     args.accumulate = accumulate_partials ? 1 : 0;
     args.h = dt;
+    args.c = c; args.c_grad = c_grad; args.qdd = qdd_out;
     args.vec_ok = aligned16(q, qd, f, g_qdd, q_grad, qd_grad, f_grad);
 
     auto bytes_of = [&](int t) { return (size_t)AbaBwdSmem(t, prog.n_dofs, prog.n_links).total_floats * sizeof(float); };
@@ -610,7 +644,18 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
     const bool need_table = table_grad != nullptr;
 #define DRM_LAUNCH_ABAB(NT, TT, IM) \
     rc = launch_persistent<aba_backward_kernel<NT, TT, IM>>(TT < 32 ? 32 : TT, smem_bytes, tiles, stream, "aba backward", &grid, prog, args)
-    if (flags & DRMB200_IMPLICIT_DAMPING) {
+#define DRM_LAUNCH_ABAB_ADDEND(NT, TT, IM) \
+    rc = launch_persistent<aba_backward_addend_kernel<NT, TT, IM>>(TT < 32 ? 32 : TT, smem_bytes, tiles, stream, "aba backward", \
+                                                                    &grid, prog, args)
+    if (c != nullptr) {
+        if (flags & DRMB200_IMPLICIT_DAMPING) {
+            if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB_ADDEND(true, 32, true); else DRM_LAUNCH_ABAB_ADDEND(true, 16, true); }
+            else            { if (tile == 32) DRM_LAUNCH_ABAB_ADDEND(false, 32, true); else DRM_LAUNCH_ABAB_ADDEND(false, 16, true); }
+        } else {
+            if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB_ADDEND(true, 32, false); else DRM_LAUNCH_ABAB_ADDEND(true, 16, false); }
+            else            { if (tile == 32) DRM_LAUNCH_ABAB_ADDEND(false, 32, false); else DRM_LAUNCH_ABAB_ADDEND(false, 16, false); }
+        }
+    } else if (flags & DRMB200_IMPLICIT_DAMPING) {
         if (need_table) { if (tile == 32) DRM_LAUNCH_ABAB(true, 32, true); else DRM_LAUNCH_ABAB(true, 16, true); }
         else            { if (tile == 32) DRM_LAUNCH_ABAB(false, 32, true); else DRM_LAUNCH_ABAB(false, 16, true); }
     } else {
@@ -618,8 +663,17 @@ int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float
         else            { if (tile == 32) DRM_LAUNCH_ABAB(false, 32, false); else DRM_LAUNCH_ABAB(false, 16, false); }
     }
 #undef DRM_LAUNCH_ABAB
+#undef DRM_LAUNCH_ABAB_ADDEND
     if (rc != DRMB200_OK) return rc;
     return need_table && reduce ? launch_reduce(args.partials, grid, topo, table_grad, stream) : DRMB200_OK;
+}
+
+int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,
+                                     const float* f, int64_t batch, uint32_t flags, const float* g_qdd,
+                                     float* q_grad, float* qd_grad, float* f_grad, float* table_grad, void* workspace,
+                                     cudaStream_t stream, bool accumulate_partials, bool reduce, float dt) {
+    return forward_dynamics_backward_device(topo, table, q, qd, f, batch, flags, g_qdd, q_grad, qd_grad, f_grad, table_grad,
+                                            workspace, stream, accumulate_partials, reduce, dt, nullptr, nullptr, nullptr);
 }
 
 int forward_dynamics_backward_device(const drmb200_topology_t* topo, const float* table, const float* q, const float* qd,

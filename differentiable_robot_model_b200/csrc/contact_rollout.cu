@@ -228,6 +228,7 @@ int contact_rollout_device(const drmb200_topology_t* topo, int32_t n_ee, const i
         return DRMB200_EINVAL;
     }
     rc = check_implicit_damping(flags, dt);
+    if (rc == DRMB200_OK) rc = check_implicit_gains(flags, dt, false);
     if (rc != DRMB200_OK) return rc;
     if (position_only && target_quat != nullptr) {
         set_error("target_quat must be null for position-only contacts");

@@ -31,6 +31,18 @@ inline int check_implicit_damping(uint32_t flags, float dt) {
     return DRMB200_OK;
 }
 
+// DRMB200_IMPLICIT_GAINS (include/drm_b200.h): the PD rollouts only (pd_rollout: whether the caller is one) and a finite
+// step dt > 0; without the flag, OK
+inline int check_implicit_gains(uint32_t flags, float dt, bool pd_rollout) {
+    if (!(flags & DRMB200_IMPLICIT_GAINS)) return DRMB200_OK;
+    if (!pd_rollout) { set_error("DRMB200_IMPLICIT_GAINS is for drmb200_pd_rollout(_backward) only"); return DRMB200_EINVAL; }
+    if (!(dt > 0.f && dt <= 3.40282347e38f)) {                  // NaN and inf fail too
+        set_error("dt=%g: implicit gains need a finite step > 0", (double)dt);
+        return DRMB200_EINVAL;
+    }
+    return DRMB200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // tile rules: bytes_of(t) is the dynamic shared memory of a CTA of tile t, static_bytes the kernel's static shared memory.
 // A rule returns the tile and its dynamic bytes; the caller refuses the choice (ELIMIT) when bytes + static_bytes exceeds

@@ -12,6 +12,10 @@
 // DRMB200_IMPLICIT_DAMPING: FD is the forward dynamics with implicit damping of step h = dt (rollout_implicit_kernel,
 // pd_rollout_implicit_kernel; aba_body.cuh), and each step of the adjoint runs the implicit ABA adjoint; the integrate and the element-wise step are
 // unchanged.
+// DRMB200_IMPLICIT_GAINS (PD only, stable PD): u-hat on the predicted position q + dt qd, the per-row pivot addends
+// c = dt (kd + dt kp) of the unsaturated joints in the ABA, tau_t = u - c qdd_t (pd_rollout_implicit_gains_kernel; the
+// definition is stated in include/drm_b200.h).  Its adjoint recomputes u_t and c_t in the element-wise step, runs the ABA
+// adjoint with the addends (backward_aba.cu) and adds the feedback terms of the header.
 //
 // Forward mapping: the articulated-body kernel's (aba.cu) -- one thread per configuration, T per CTA, the same per-thread
 // body (aba_body.cuh) -- with the time loop of rollout_pipeline.cuh inside (rollout_kernel: its own copy).  Once per CTA the table is staged (and folded,
@@ -42,7 +46,8 @@
 namespace drm {
 
 int forward_dynamics_backward_device(const drmb200_topology_t*, const float*, const float*, const float*, const float*, int64_t,
-                                     uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t, bool, bool, float);
+                                     uint32_t, const float*, float*, float*, float*, float*, void*, cudaStream_t, bool, bool, float,
+                                     const float*, float*, float*);
 int64_t forward_dynamics_backward_workspace_bytes(const drmb200_topology_t*, int64_t);
 
 // u = (f + kp e) + kd ed with e = q_ref - q, ed = qd_ref - qd: the rounding of the torch expression
@@ -229,9 +234,10 @@ struct PDRolloutArgs {
 };
 
 struct PDRolloutSmem {
-    int q, qd, in, tau, qdd, kp, kd, lim, table, link, slots, total_floats;
-    // n_in input tiles per step (q_ref, then qd_ref and f when given); every region starts 16-byte aligned
-    __host__ __device__ PDRolloutSmem(int T, int n, int n_links, int n_slots, int n_in, bool per_row) {
+    int q, qd, in, tau, qdd, kp, kd, lim, table, link, slots, piv, total_floats;
+    // n_in input tiles per step (q_ref, then qd_ref and f when given); every region starts 16-byte aligned.  gains: the
+    // implicit gains' per-row pivot addends c of the current step, [T, n] after every other region (empty without)
+    __host__ __device__ PDRolloutSmem(int T, int n, int n_links, int n_slots, int n_in, bool per_row, bool gains = false) {
         const int gain = ((per_row ? T : 1) * n + 3) & ~3;
         int o = 0;
         q = o;   o += T * n;
@@ -245,13 +251,16 @@ struct PDRolloutSmem {
         table = o; o += n_links * DRMB200_TABLE_STRIDE;
         link = o;  o += n_links * ABA_LINK * T;
         slots = o; o += n_slots * ABA_SLOT * T;
+        piv = o;   o += gains ? T * n : 0;
         total_floats = o;
     }
 };
 
-// The PD kernel's body, instantiated by pd_rollout_kernel (explicit damping) and pd_rollout_implicit_kernel: two kernel
-// names rather than a template flag on one, so that the explicit kernel keeps its symbol.
-template <int T, bool IMPLICIT>
+// The PD kernel's body, instantiated by pd_rollout_kernel (explicit damping), pd_rollout_implicit_kernel and
+// pd_rollout_implicit_gains_kernel: kernel names rather than a template flag on one, so that the explicit kernel keeps its
+// symbol.  GAINS (DRMB200_IMPLICIT_GAINS): each thread forms u_t into its tau row and c_t into its row of the addend tile,
+// the ABA runs with the pivot addends c_t, and the tau row then becomes u_t - c_t qdd_t on the unsaturated joints.
+template <int T, bool IMPLICIT, bool GAINS = false>
 __device__ __forceinline__ void pd_rollout_run(const TreeProgram& prog, const FoldProgram& fold, const PDRolloutArgs args) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar[2];
@@ -259,7 +268,7 @@ __device__ __forceinline__ void pd_rollout_run(const TreeProgram& prog, const Fo
     const int n = prog.n_dofs;
     const bool has_qdr = args.qd_ref != nullptr, has_f = args.f != nullptr, has_lim = args.lim != nullptr;
     const int n_in = 1 + (int)has_qdr + (int)has_f;
-    const PDRolloutSmem L(T, n, prog.n_links, prog.n_slots, n_in, args.per_row != 0);
+    const PDRolloutSmem L(T, n, prog.n_links, prog.n_slots, n_in, args.per_row != 0, GAINS);
     float* s_tau = smem + L.tau;
     float* s_qdd = smem + L.qdd;
     float* s_kp = smem + L.kp;
@@ -296,13 +305,35 @@ __device__ __forceinline__ void pd_rollout_run(const TreeProgram& prog, const Fo
             const float* qdr = pipe.s_qd + tid * n;
             const float* ref = s_it + tid * n;
             float* taur = s_taut + tid * n;
-            for (int k = 0; k < n; ++k) {
-                float e, ed;
-                const float u = pd_command(ref[k], qr[k], has_qdr ? ref[T * n + k] : 0.f, qdr[k], has_f ? ref[o_f + k] : 0.f,
-                                           s_kp[gain_row + k], s_kd[gain_row + k], e, ed);
-                taur[k] = has_lim ? pd_clamp(u, s_lim[k]) : u;
+            if constexpr (GAINS) {
+                const float h = args.dt;
+                float* cr = smem + L.piv + tid * n;
+                float* ar = s_qddt + tid * n;
+                uint64_t sat = 0;                                // n <= 63
+                for (int k = 0; k < n; ++k) {
+                    const float kp = s_kp[gain_row + k], kd = s_kd[gain_row + k];
+                    const float qp = __fadd_rn(qr[k], __fmul_rn(h, qdr[k]));      // the position the step predicts
+                    float e, ed;
+                    const float u = pd_command(ref[k], qp, has_qdr ? ref[T * n + k] : 0.f, qdr[k], has_f ? ref[o_f + k] : 0.f,
+                                               kp, kd, e, ed);
+                    const bool s = has_lim && !(u >= -s_lim[k] && u <= s_lim[k]);   // torch.clamp's rule, NaN saturated
+                    sat |= (uint64_t)s << k;
+                    taur[k] = s ? pd_clamp(u, s_lim[k]) : u;
+                    cr[k] = s ? 0.f : __fmul_rn(h, __fadd_rn(kd, __fmul_rn(h, kp)));
+                }
+                aba_body<T, IMPLICIT, true>(prog, s_tab, qr, qdr, taur, ar, s_link + tid, s_slot + tid, args.flags, h, cr);
+                for (int k = 0; k < n; ++k)
+                    if (!((sat >> k) & 1)) taur[k] = __fsub_rn(taur[k], __fmul_rn(cr[k], ar[k]));
+            } else {
+                for (int k = 0; k < n; ++k) {
+                    float e, ed;
+                    const float u = pd_command(ref[k], qr[k], has_qdr ? ref[T * n + k] : 0.f, qdr[k], has_f ? ref[o_f + k] : 0.f,
+                                               s_kp[gain_row + k], s_kd[gain_row + k], e, ed);
+                    taur[k] = has_lim ? pd_clamp(u, s_lim[k]) : u;
+                }
+                aba_body<T, IMPLICIT>(prog, s_tab, qr, qdr, taur, s_qddt + tid * n, s_link + tid, s_slot + tid, args.flags,
+                                      args.dt);
             }
-            aba_body<T, IMPLICIT>(prog, s_tab, qr, qdr, taur, s_qddt + tid * n, s_link + tid, s_slot + tid, args.flags, args.dt);
         }
         pipe.integrate_and_store(t, s_qddt + tid * n, 1, args.tau, s_taut, args.qdd, s_qddt);
     }
@@ -320,6 +351,14 @@ __global__ void __launch_bounds__(T)
 pd_rollout_implicit_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold,
                            const PDRolloutArgs args) {
     pd_rollout_run<T, true>(prog, fold, args);
+}
+
+// DRMB200_IMPLICIT_GAINS, with explicit (IMPLICIT = false) or implicit joint damping
+template <int T, bool IMPLICIT>
+__global__ void __launch_bounds__(T)
+pd_rollout_implicit_gains_kernel(const __grid_constant__ TreeProgram prog, const __grid_constant__ FoldProgram fold,
+                                 const PDRolloutArgs args) {
+    pd_rollout_run<T, IMPLICIT, true>(prog, fold, args);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -362,14 +401,64 @@ struct AdjStepArgs {
     float dt;
     int32_t first;              // t = T - 1: the running adjoints start at zero
     int32_t final;              // after step 0: post-update only, written to out_q / out_qd
+    // implicit gains: the pivot adjoint c-bar and the accelerations of step s (the ABA adjoint's outputs); step t's state,
+    // inputs and upstream g_tau, and its u_t / c_t for the ABA adjoint (written)
+    const float* c_bar;
+    const float* qdd_s;
+    const float* qt;
+    const float* qdt;
+    const float* q_ref_t;
+    const float* qd_ref_t;
+    const float* f_t;
+    const float* g_tau_t;
+    float* u_step;
+    float* c_step;
 };
 
-template <bool Feedback>
-__global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStepArgs a) {
+// The implicit gains' command of a step (drmb200_pd_rollout, DRMB200_IMPLICIT_GAINS) at element i: u-hat on the predicted
+// position q + h qd, whether it saturates (torch.clamp's rule, NaN saturated) and its e, ed.  q_ref / qd_ref / f / lim are
+// the step's (qd_ref / f / lim may be NULL).
+__device__ __forceinline__ float pd_gains_command(const AdjStepArgs& a, int64_t i, const float* q, const float* qd,
+                                                  const float* q_ref, const float* qd_ref, const float* f, float kp, float kd,
+                                                  float& e, float& ed, bool& sat) {
+    const int k = (int)(i % a.n);
+    const float qp = __fadd_rn(q[i], __fmul_rn(a.dt, qd[i]));
+    const float u = pd_command(q_ref[i], qp, qd_ref ? qd_ref[i] : 0.f, qd[i], f ? f[i] : 0.f, kp, kd, e, ed);
+    sat = a.lim != nullptr && !(u >= -a.lim[k] && u <= a.lim[k]);
+    return u;
+}
+
+// Gains (only with Feedback): the adjoint of the implicit gains.  The pre-update of step t also recomputes u_t, c_t (for
+// the ABA adjoint) and adds -c_t g_tau[t] to g_qdd_t; the post-update of step s takes, with gu = mask (gf + g_tau) and
+// gc = mask (c-bar - qdd_s g_tau), a_q -= kp gu, a_qd -= (kd + h kp) gu, f_grad = gu, q_ref_grad = kp gu,
+// qd_ref_grad = kd gu, kp_grad += gu e + h^2 gc, kd_grad += gu ed + h gc.
+template <bool Feedback, bool Gains>
+__device__ __forceinline__ void rollout_adjoint_step(const AdjStepArgs& a) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.count; i += (int64_t)gridDim.x * blockDim.x) {
         float aq = 0.f, aqd = 0.f;
         if (!a.first) {                                        // post-update of step s
-            if constexpr (Feedback) {
+            if constexpr (Gains) {
+                const int64_t gi = a.per_row ? i : (int)(i % a.n);
+                const float kp = a.kp[gi], kd = a.kd[gi], h = a.dt;
+                float e, ed;
+                bool sat;
+                pd_gains_command(a, i, a.qs, a.qds, a.q_ref, a.qd_ref, a.f, kp, kd, e, ed, sat);
+                float gu = a.gf[i], gc = a.c_bar[i];
+                if (a.g_tau != nullptr) {
+                    gu = __fadd_rn(gu, a.g_tau[i]);
+                    gc = __fsub_rn(gc, __fmul_rn(a.qdd_s[i], a.g_tau[i]));
+                }
+                if (sat) gu = gc = 0.f;
+                aq = __fsub_rn(__fadd_rn(a.a_q[i], a.gq[i]), __fmul_rn(kp, gu));
+                aqd = __fsub_rn(__fadd_rn(a.a_qd[i], a.gqd[i]), __fmul_rn(__fadd_rn(kd, __fmul_rn(h, kp)), gu));
+                if (a.f_grad != nullptr) a.f_grad[i] = gu;
+                if (a.q_ref_grad != nullptr) a.q_ref_grad[i] = __fmul_rn(kp, gu);
+                if (a.qd_ref_grad != nullptr) a.qd_ref_grad[i] = __fmul_rn(kd, gu);
+                const float gkp = __fadd_rn(__fmul_rn(gu, e), __fmul_rn(__fmul_rn(h, h), gc));
+                const float gkd = __fadd_rn(__fmul_rn(gu, ed), __fmul_rn(h, gc));
+                if (a.kp_grad != nullptr) a.kp_grad[i] = a.last_post ? gkp : __fadd_rn(a.kp_grad[i], gkp);
+                if (a.kd_grad != nullptr) a.kd_grad[i] = a.last_post ? gkd : __fadd_rn(a.kd_grad[i], gkd);
+            } else if constexpr (Feedback) {
                 const int k = (int)(i % a.n);
                 const int64_t gi = a.per_row ? i : k;
                 const float kp = a.kp[gi], kd = a.kd[gi];
@@ -401,22 +490,44 @@ __global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStep
         aqd = __fadd_rn(aqd, __fmul_rn(a.dt, aq));             // a_qd' = a_qd + dt a_q
         float g = __fmul_rn(a.dt, aqd);
         if (a.g_qdd != nullptr) g = __fadd_rn(g, a.g_qdd[i]);
+        if constexpr (Gains) {                                 // u_t, c_t as the forward formed them
+            const int k = (int)(i % a.n);
+            const int64_t gi = a.per_row ? i : k;
+            const float kp = a.kp[gi], kd = a.kd[gi], h = a.dt;
+            float e, ed;
+            bool sat;
+            const float u = pd_gains_command(a, i, a.qt, a.qdt, a.q_ref_t, a.qd_ref_t, a.f_t, kp, kd, e, ed, sat);
+            const float c = sat ? 0.f : __fmul_rn(h, __fadd_rn(kd, __fmul_rn(h, kp)));
+            a.u_step[i] = sat ? pd_clamp(u, a.lim[k]) : u;
+            a.c_step[i] = c;
+            if (a.g_tau_t != nullptr) g = __fsub_rn(g, __fmul_rn(c, a.g_tau_t[i]));
+        }
         a.a_q[i] = aq;
         a.a_qd[i] = aqd;
         a.g_step[i] = g;
     }
 }
 
+template <bool Feedback>
+__global__ void __launch_bounds__(256) rollout_adjoint_step_kernel(const AdjStepArgs a) {
+    rollout_adjoint_step<Feedback, false>(a);
+}
+
+__global__ void __launch_bounds__(256) pd_rollout_implicit_gains_adjoint_step_kernel(const AdjStepArgs a) {
+    rollout_adjoint_step<true, true>(a);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-// "rnea_fold", as drmb200_forward_dynamics, and the checks both forward rollouts start with
+// "rnea_fold", as drmb200_forward_dynamics, and the checks both forward rollouts start with (pd: the PD rollout's)
 static int rollout_program(const drmb200_topology_t* topo, int64_t batch, int32_t n_steps, float dt, uint32_t flags,
-                           FoldChoice* fc) {
+                           bool pd, FoldChoice* fc) {
     const int rc = select_fold(topo, false, fc);
     if (rc != DRMB200_OK) return rc;
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
-    return check_implicit_damping(flags, dt);
+    const int rd = check_implicit_damping(flags, dt);
+    return rd != DRMB200_OK ? rd : check_implicit_gains(flags, dt, pd);
 }
 
 // 64 configurations per CTA when that still gives every SM a CTA and the per-link state leaves room for two CTAs per SM;
@@ -454,7 +565,7 @@ int forward_dynamics_rollout_device(const drmb200_topology_t* topo, const float*
                                     const float* f, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q,
                                     float* qd, float* qdd, cudaStream_t stream) {
     FoldChoice fc;
-    const int rc = rollout_program(topo, batch, n_steps, dt, flags, &fc);
+    const int rc = rollout_program(topo, batch, n_steps, dt, flags, false, &fc);
     if (rc != DRMB200_OK) return rc;
     const TreeProgram& prog = *fc.prog;
     if (batch == 0 || n_steps == 0 || prog.n_dofs == 0) return DRMB200_OK;
@@ -475,7 +586,7 @@ int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const 
                       const float* effort_limit, int64_t batch, int32_t n_steps, float dt, uint32_t flags, float* q, float* qd,
                       float* qdd, float* tau, cudaStream_t stream) {
     FoldChoice fc;
-    const int rc = rollout_program(topo, batch, n_steps, dt, flags, &fc);
+    const int rc = rollout_program(topo, batch, n_steps, dt, flags, true, &fc);
     if (rc != DRMB200_OK) return rc;
     const TreeProgram& prog = *fc.prog;
     if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
@@ -493,6 +604,18 @@ int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const 
     args.aligned = aligned16(q0, qd0, q_ref, qd_ref, f, q, qd, qdd, tau) && (!gains_per_row || aligned16(kp, kd)) &&
                    ((batch * prog.n_dofs) & 3) == 0;
     const int n_in = 1 + (qd_ref != nullptr) + (f != nullptr);
+    if (flags & DRMB200_IMPLICIT_GAINS) {
+        auto gains_floats_of = [&](int T) {
+            return PDRolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots, n_in, gains_per_row != 0, true).total_floats;
+        };
+        if (flags & DRMB200_IMPLICIT_DAMPING)
+            return launch_rollout<pd_rollout_implicit_gains_kernel<64, true>, pd_rollout_implicit_gains_kernel<32, true>,
+                                  pd_rollout_implicit_gains_kernel<16, true>>(fc, batch, gains_floats_of, "pd rollout", args,
+                                                                              stream);
+        return launch_rollout<pd_rollout_implicit_gains_kernel<64, false>, pd_rollout_implicit_gains_kernel<32, false>,
+                              pd_rollout_implicit_gains_kernel<16, false>>(fc, batch, gains_floats_of, "pd rollout", args,
+                                                                           stream);
+    }
     auto floats_of = [&](int T) {
         return PDRolloutSmem(T, prog.n_dofs, prog.n_links, prog.n_slots, n_in, gains_per_row != 0).total_floats;
     };
@@ -504,11 +627,12 @@ int pd_rollout_device(const drmb200_topology_t* topo, const float* table, const 
 }
 
 // The reverse-time adjoint of both rollouts.  Workspace: [ABA adjoint workspace | a_q | a_qd | g_qdd_t | gq | gqd (| gf
-// with feedback)], each [B, n] fp32.
+// with feedback | u_t | c_t | c-bar | qdd for the implicit gains)], each [B, n] fp32.  The feedback bound covers the
+// implicit gains, with or without them.
 int64_t rollout_adjoint_workspace_bytes(const drmb200_topology_t* topo, int64_t batch, bool feedback) {
     if (topo == nullptr || topo->n_links < 1 || topo->n_links > DRMB200_MAX_LINKS || batch < 0) return 0;
     return round256(forward_dynamics_backward_workspace_bytes(topo, batch)) +
-           (feedback ? 6 : 5) * round256(batch * topo->n_dofs * (int64_t)sizeof(float));
+           (feedback ? 10 : 5) * round256(batch * topo->n_dofs * (int64_t)sizeof(float));
 }
 
 // tau: the [T, B, n] torques the forward applied.  Open loop (fb == NULL): f_grad receives the ABA adjoint's f gradient.
@@ -531,10 +655,18 @@ static int rollout_adjoint(const drmb200_topology_t* topo, const float* table, c
     float* gq = reinterpret_cast<float*>(ws + 3 * slice);
     float* gqd = reinterpret_cast<float*>(ws + 4 * slice);
     float* gf = fb ? reinterpret_cast<float*>(ws + 5 * slice) : nullptr;
+    const bool gains = fb != nullptr && (flags & DRMB200_IMPLICIT_GAINS);
+    float* u_step = gains ? reinterpret_cast<float*>(ws + 6 * slice) : nullptr;
+    float* c_step = gains ? reinterpret_cast<float*>(ws + 7 * slice) : nullptr;
+    float* c_bar = gains ? reinterpret_cast<float*>(ws + 8 * slice) : nullptr;
+    float* qdd_s = gains ? reinterpret_cast<float*>(ws + 9 * slice) : nullptr;
 
     int64_t blocks = (count + 255) / 256;
     if (blocks > (int64_t)device_sm_count() * 8) blocks = (int64_t)device_sm_count() * 8;
     auto step_kernel = [&](const AdjStepArgs& a) {
+        if (gains)
+            return launch_kernel<pd_rollout_implicit_gains_adjoint_step_kernel>(blocks, 256, 0, stream, false,
+                                                                                "pd rollout adjoint step", a);
         return fb ? launch_kernel<rollout_adjoint_step_kernel<true>>(blocks, 256, 0, stream, false, "pd rollout adjoint step", a)
                   : launch_kernel<rollout_adjoint_step_kernel<false>>(blocks, 256, 0, stream, false, "rollout adjoint step", a);
     };
@@ -543,6 +675,7 @@ static int rollout_adjoint(const drmb200_topology_t* topo, const float* table, c
     AdjStepArgs a = fb ? *fb : AdjStepArgs{};
     a.a_q = a_q; a.a_qd = a_qd; a.g_step = g_step; a.gq = gq; a.gqd = gqd; a.gf = gf;
     a.n = topo->n_dofs; a.count = count; a.dt = dt;
+    a.c_bar = c_bar; a.qdd_s = qdd_s; a.u_step = u_step; a.c_step = c_step;
     // the feedback post-update of step s reads its state (q0 / qd0, then the forward's outputs) and inputs, writes its
     // gradients
     auto post = [&](int s) {
@@ -560,13 +693,19 @@ static int rollout_adjoint(const drmb200_topology_t* topo, const float* table, c
         a.g_q = at(g_q, t);
         a.g_qd = at(g_qd, t);
         a.g_qdd = at(g_qdd, t);
-        int rc = step_kernel(a);
-        if (rc != DRMB200_OK) return rc;
         const float* qt = t == 0 ? q0 : q + (int64_t)(t - 1) * count;     // step inputs: (q0, qd0), then the forward's outputs
         const float* qdt = t == 0 ? qd0 : qd + (int64_t)(t - 1) * count;
-        rc = forward_dynamics_backward_device(topo, table, qt, qdt, tau + (int64_t)t * count, batch, flags, g_step, gq, gqd,
-                                              fb ? gf : at(f_grad, t), table_grad, fd_ws, stream,
-                                              /*accumulate_partials=*/t != n_steps - 1, /*reduce=*/t == 0, dt);
+        if (gains) {
+            a.qt = qt; a.qdt = qdt;
+            a.q_ref_t = at(fb->q_ref, t); a.qd_ref_t = at(fb->qd_ref, t); a.f_t = at(fb->f, t); a.g_tau_t = at(fb->g_tau, t);
+        }
+        int rc = step_kernel(a);
+        if (rc != DRMB200_OK) return rc;
+        // the implicit gains' ABA ran on u_t with the pivot addends c_t (the pre-update just wrote both), not on tau_t
+        rc = forward_dynamics_backward_device(topo, table, qt, qdt, gains ? u_step : tau + (int64_t)t * count, batch, flags,
+                                              g_step, gq, gqd, fb ? gf : at(f_grad, t), table_grad, fd_ws, stream,
+                                              /*accumulate_partials=*/t != n_steps - 1, /*reduce=*/t == 0, dt, c_step, c_bar,
+                                              qdd_s);
         if (rc != DRMB200_OK) return rc;
     }
     if (!want_final) return DRMB200_OK;
@@ -590,6 +729,7 @@ int forward_dynamics_rollout_backward_device(const drmb200_topology_t* topo, con
     if (topo == nullptr) { set_error("null topology"); return DRMB200_EINVAL; }
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
     if (check_implicit_damping(flags, dt) != DRMB200_OK) return DRMB200_EINVAL;
+    if (check_implicit_gains(flags, dt, false) != DRMB200_OK) return DRMB200_EINVAL;
     if (batch == 0 || n_steps == 0 || topo->n_dofs == 0) return DRMB200_OK;
     if (q0_grad == nullptr && qd0_grad == nullptr && f_grad == nullptr && table_grad == nullptr) return DRMB200_OK;
     if (table == nullptr || q0 == nullptr || qd0 == nullptr || f == nullptr || (n_steps > 1 && (q == nullptr || qd == nullptr))) {
@@ -615,6 +755,7 @@ int pd_rollout_backward_device(const drmb200_topology_t* topo, const float* tabl
     if (topo == nullptr) { set_error("null topology"); return DRMB200_EINVAL; }
     if (batch < 0 || n_steps < 0) { set_error("batch=%lld, n_steps=%d: must be >= 0", (long long)batch, (int)n_steps); return DRMB200_EINVAL; }
     if (check_implicit_damping(flags, dt) != DRMB200_OK) return DRMB200_EINVAL;
+    if (check_implicit_gains(flags, dt, true) != DRMB200_OK) return DRMB200_EINVAL;
     if (gains_per_row != 0 && gains_per_row != 1) { set_error("gains_per_row=%d: must be 0 or 1", (int)gains_per_row); return DRMB200_EINVAL; }
     if (batch == 0 || n_steps == 0 || topo->n_dofs == 0) return DRMB200_OK;
     const bool want_elementwise = q0_grad || qd0_grad || q_ref_grad || qd_ref_grad || f_grad || kp_grad || kd_grad;

@@ -24,6 +24,7 @@ GRAVITY = 1
 DAMPING = 2
 INERTIAL_GRADS_ONLY = 4      # backward hint: no kinematic link parameter is learnable (see include/drm_b200.h)
 IMPLICIT_DAMPING = 8         # rollouts: the damping torque taken at the end-of-step velocity (see include/drm_b200.h)
+IMPLICIT_GAINS = 16          # PD rollout: the PD law taken at the end-of-step state, stable PD (see include/drm_b200.h)
 
 _c_float_p = ctypes.c_void_p      # raw device / host addresses
 _SIGNATURES = {
@@ -459,8 +460,9 @@ def forward_dynamics_rollout_raw(topo, table, q0, qd0, f, dt, flags, want_qdd=Tr
 
 def pd_rollout_raw(topo, table, q0, qd0, q_ref, kp, kd, dt, flags, qd_ref=None, f=None, effort_limit=None, want_qdd=True):
     """(q, qd, qdd, tau) [T, B, n] of T semi-implicit Euler steps over the articulated-body algorithm driven by the PD law
-    tau = clamp(f + kp (q_ref - q) + kd (qd_ref - qd), -effort_limit, effort_limit), one launch (drmb200_pd_rollout).
-    kp / kd both [n] (shared) or both [B, n] (per row); qd_ref, f, effort_limit may be None; qdd is None unless want_qdd."""
+    tau = clamp(f + kp (q_ref - q) + kd (qd_ref - qd), -effort_limit, effort_limit), one launch (drmb200_pd_rollout;
+    IMPLICIT_GAINS in flags: the law at the end-of-step state).  kp / kd both [n] (shared) or both [B, n] (per row); qd_ref,
+    f, effort_limit may be None; qdd is None unless want_qdd."""
     _require_cuda(table, q0, qd0, q_ref, kp, kd, qd_ref, f, effort_limit)
     if kp.shape != kd.shape:      # one gains_per_row flag describes both buffers
         raise RuntimeError(f"kp and kd must have the same shape (got {tuple(kp.shape)} and {tuple(kd.shape)})")

@@ -1083,6 +1083,7 @@ class DifferentiableRobotModel(torch.nn.Module):
         include_gravity: Optional[bool] = True,
         use_damping: Optional[bool] = False,
         implicit_damping: bool = False,
+        implicit_gains: bool = False,
     ) -> ControlledRollout:
         r"""Simulate a joint-space PD controller tracking reference trajectories: :meth:`compute_forward_dynamics_rollout`
         with the torque of every step computed from the current state, all ``T`` steps in ONE launch
@@ -1098,6 +1099,24 @@ class DifferentiableRobotModel(torch.nn.Module):
         ``use_damping``) the loop's call is ``compute_forward_dynamics(q, qd, u, ..., implicit_damping_dt=dt)``, stable in
         the joint damping at any ``dt``.
 
+        The explicit step is stable only for gains inside its own limits: for one joint of inertia ``I``, with
+        ``a = dt**2 kp / I`` and ``b = dt kd / I``, it needs ``b < 2`` and ``a + 2 b < 4`` (about ``dt * sqrt(kp / I) < 0.83``
+        at critical damping).  ``implicit_gains=True`` (stable PD) takes the PD law at the end-of-step state instead::
+
+            qp = q + dt * qd                                            # the position the step predicts
+            u = f[t] + kp * (q_ref[t] - qp) + kd * (qd_ref[t] - qd)
+            sat = ~(-effort_limit <= u <= effort_limit)                 # all False without a limit; NaN saturates
+            u = torch.where(sat, torch.clamp(u, -effort_limit, effort_limit), u)
+            c = torch.where(sat, 0, dt * (kd + dt * kp))
+            qdd = forward dynamics of (q, qd, u) with every joint's articulated-body pivot + c    # (H + diag(c)) qdd = u - nle
+            tau = torch.where(sat, u, u - c * qdd)
+
+        so that on an unsaturated joint ``tau = f + kp (q_ref - q_next) + kd (qd_ref - qd_next)`` (the law at the state the
+        step ends in, up to rounding), and the step is stable at every ``dt`` for ``kp, kd >= 0``; the signs are not checked.
+        The effort limit is decided on the predicted command: a saturated joint gets the clamped torque, and an unsaturated
+        joint's applied ``tau`` can exceed the limit by ``|c * qdd|``.  It combines with ``implicit_damping``
+        (``include/drm_b200.h``: ``DRMB200_IMPLICIT_GAINS``).
+
         Args:
             q0, qd0: initial joint angles / velocities [batch_size x n_dofs] (or [n_dofs])
             q_ref: reference joint angles of every step [T x batch_size x n_dofs] (or [T x n_dofs])
@@ -1108,6 +1127,8 @@ class DifferentiableRobotModel(torch.nn.Module):
             f: feed-forward joint forces, shaped like ``q_ref``; None: zero; never modified
             effort_limit: symmetric torque limit [n_dofs], every entry > 0 (``inf`` allowed); None: no limit.
                 ``get_joint_limits()[i]["effort"]`` is a natural choice, but some shipped URDFs list 0 there.
+            implicit_damping: take the joint damping implicitly with step ``dt`` (needs ``use_damping``)
+            implicit_gains: take the PD law at the end-of-step state (stable PD, above; needs a finite ``dt > 0``)
         Returns: :class:`ControlledRollout` ``(q, qd, qdd, tau)``, each [T x batch_size x n_dofs] (or [T x n_dofs]), with
         ``q[t] = q_{t+1}``, ``qd[t] = qd_{t+1}``, ``qdd[t] = qdd_t`` and ``tau[t]`` the torque applied at step ``t``.
         Differentiable w.r.t. q0, qd0, q_ref, qd_ref, f, kp, kd and every learnable link parameter (the articulated-body
@@ -1134,8 +1155,11 @@ class DifferentiableRobotModel(torch.nn.Module):
             q0, qd0, q_ref, qd_ref, f = self._rollout_batch_dim(q0, qd0, q_ref, qd_ref, f)
         flags = (engine.GRAVITY if include_gravity else 0) | (engine.DAMPING if use_damping else 0)
         flags |= engine.IMPLICIT_DAMPING if implicit_damping else 0
+        flags |= engine.IMPLICIT_GAINS if implicit_gains else 0
         table = self._link_table()
         dt = self._implicit_damping_step(implicit_damping, use_damping, dt)
+        if implicit_gains:
+            assert 0.0 < dt < float("inf"), f"implicit gains need a finite step dt > 0 (got {dt})"
         lim = None if effort_limit is None else effort_limit.detach()
         if kp.shape != kd.shape:
             # the kernel reads both gains in one layout: the shared one becomes a per-row view (its gradient is the sum of

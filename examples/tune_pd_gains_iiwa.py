@@ -8,7 +8,14 @@ w = 10 rad/s, zeta = 1 on every joint.  The learning rate bounds how far they mo
 inside the region where semi-implicit Euler is stable.  The torques are clamped to a limit proportional to each
 joint's inertia, so that raising the gains without bound stops paying off.
 
-    python examples/tune_pd_gains_iiwa.py [--batch 256] [--steps 200] [--iters 100] [--json]
+With ``--implicit-gains`` the rollout takes the PD law at the end-of-step state (stable PD,
+``compute_pd_controlled_rollout(..., implicit_gains=True)``), which is stable at every dt for any non-negative gains, and
+the tuning starts instead from w = 2000 rad/s, zeta = 1: dt w = 1.95, far past the explicit step's limit of about 0.83
+at critical damping, where the default rollout is non-finite.  It runs without the torque limit and at a larger learning
+rate: from such gains every joint would start saturated, where the limit passes no gradient, and the torque cost alone
+keeps the gains from growing.
+
+    python examples/tune_pd_gains_iiwa.py [--batch 256] [--steps 200] [--iters 100] [--implicit-gains] [--json]
 """
 import argparse
 import json
@@ -19,7 +26,8 @@ import torch
 from differentiable_robot_model_b200 import DifferentiableKUKAiiwa
 
 
-def run(batch=256, steps=200, iters=100, dt=2.0 ** -10, effort_weight=1e-6, lr=0.03, device="cuda:0", log=print):
+def run(batch=256, steps=200, iters=100, dt=2.0 ** -10, effort_weight=1e-6, lr=0.03, device="cuda:0", log=print,
+        implicit_gains=False):
     torch.manual_seed(0)
     robot = DifferentiableKUKAiiwa(device=device)
     limits = robot.get_joint_limits()
@@ -34,16 +42,19 @@ def run(batch=256, steps=200, iters=100, dt=2.0 ** -10, effort_weight=1e-6, lr=0
     q_ref = q0 + amp * torch.sin(freq * s)
     qd_ref = amp * freq * torch.cos(freq * s)
     inertia = torch.diagonal(robot.compute_lagrangian_inertia_matrix(q0), dim1=1, dim2=2).mean(0)
-    effort_limit = 2000.0 * inertia
-    log_kp = torch.full((n,), math.log(10.0 ** 2), device=device, requires_grad=True)      # w = 10 rad/s
-    log_kd = torch.full((n,), math.log(2 * 1.0 * 10.0), device=device, requires_grad=True)  # zeta = 1
+    effort_limit = None if implicit_gains else 2000.0 * inertia
+    lr = 0.1 if implicit_gains else lr
+    w0 = 2000.0 if implicit_gains else 10.0                                                 # rad/s
+    log_kp = torch.full((n,), math.log(w0 ** 2), device=device, requires_grad=True)
+    log_kd = torch.full((n,), math.log(2 * 1.0 * w0), device=device, requires_grad=True)    # zeta = 1
     opt = torch.optim.Adam([log_kp, log_kd], lr=lr)
     hist = []
     for it in range(iters):
         opt.zero_grad()
         q, _, _, tau = robot.compute_pd_controlled_rollout(q0, torch.zeros_like(q0), q_ref, log_kp.exp() * inertia,
                                                            log_kd.exp() * inertia, dt,
-                                                           qd_ref=qd_ref, effort_limit=effort_limit)
+                                                           qd_ref=qd_ref, effort_limit=effort_limit,
+                                                           implicit_gains=implicit_gains)
         tracking = ((q - q_ref) ** 2).mean()
         cost = tracking + effort_weight * (tau ** 2).mean()
         cost.backward()
@@ -59,10 +70,12 @@ def main():
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--iters", type=int, default=100)
+    ap.add_argument("--implicit-gains", action="store_true",
+                    help="stable PD: the law at the end-of-step state, tuned from w = 2000 rad/s")
     ap.add_argument("--json", action="store_true", help="print one JSON line with the results")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "this example runs the CUDA engine and needs a GPU"
-    hist, kp, kd = run(args.batch, args.steps, args.iters)
+    hist, kp, kd = run(args.batch, args.steps, args.iters, implicit_gains=args.implicit_gains)
     print(f"cost {hist[0]:.3e} -> {hist[-1]:.3e}; kp {[round(v, 1) for v in kp.tolist()]}, kd {[round(v, 2) for v in kd.tolist()]}")
     if args.json:
         print(json.dumps({"first_cost": hist[0], "last_cost": hist[-1], "kp": kp.tolist(), "kd": kd.tolist()}))

@@ -93,6 +93,10 @@ extern "C" {
  * implicit joint damping with step h = dt, as defined at drmb200_forward_dynamics_implicit_damping.  Needs
  * DRMB200_DAMPING and a finite dt > 0, else DRMB200_EINVAL. */
 #define DRMB200_IMPLICIT_DAMPING 8u
+/* drmb200_pd_rollout(_backward) only: implicit PD gains (stable PD) with step h = dt, as defined at drmb200_pd_rollout.
+ * Needs a finite dt > 0, else DRMB200_EINVAL; combines freely with DRMB200_IMPLICIT_DAMPING.  The other rollouts return
+ * DRMB200_EINVAL for it. */
+#define DRMB200_IMPLICIT_GAINS 16u
 
 /*
  * Immutable kinematic-tree topology, host memory, links in URDF document order
@@ -352,6 +356,27 @@ int drmb200_forward_dynamics_rollout_backward(const drmb200_topology_t* topo, co
  * no-op.  DRMB200_EINVAL for a NULL required pointer or a negative size.  A CTA holds 64 or 32 configurations, or 16 when
  * 32 need more than 227 KB of shared memory (per-row gains and all three input streams take a 63-DoF chain there);
  * DRMB200_ELIMIT only when a 16-configuration CTA still needs more (the message names the bytes).
+ *
+ * DRMB200_IMPLICIT_GAINS (stable PD; needs a finite dt > 0, combines with DRMB200_IMPLICIT_DAMPING): the PD law is taken
+ * at the end-of-step state.  With h = dt, step t computes, every operation rounded separately (no FMA but the pivot's):
+ *     qp     = q_t + h * qd_t                            the position the step predicts at the current velocity
+ *     e      = q_ref[t] - qp;   ed = qd_ref[t] - qd_t     (qd_ref NULL: 0.f - qd_t)
+ *     u^     = (f[t] + kp * e) + kd * ed                 (f NULL: 0.f + kp * e)
+ *     sat    = effort_limit given and !(-lim <= u^ <= lim)   torch.clamp's rule; NaN counts as saturated
+ *     u      = sat ? clamp(u^, -lim, lim) : u^
+ *     c      = sat ? 0 : h * (kd + h * kp)               per row and joint, per step
+ *     qdd_t  = FD'(q_t, qd_t, u)    the ABA of drmb200_forward_dynamics (of drmb200_forward_dynamics_implicit_damping
+ *                                   under DRMB200_IMPLICIT_DAMPING) with every movable joint k's pivot d_k (+ h damping_k)
+ *                                   then + c_k, one rounded add
+ *     tau_t  = sat ? u : u - c * qdd_t
+ * and the integrate as above.  For a symmetric inertia (H + h D_impl + diag(h kd + h^2 kp)) qdd_t = u^ - nle, so on an
+ * unsaturated joint tau_t = f + kp (q_ref - q_{t+1}) + kd (qd_ref - qd_{t+1}) up to rounding: the PD law at the
+ * end-of-step state.  For one joint of inertia I with kp, kd >= 0 the step is stable at every h, where the explicit one
+ * needs h kd / I < 2 and h^2 kp / I + 2 h kd / I < 4.  The gains' signs are not checked (that would need a host
+ * synchronisation): negative gains may leave a pivot <= 0.  The effort limit is decided on the predicted command u^: a
+ * saturated joint gets the clamped constant torque and no pivot term, and an unsaturated joint's applied tau_t may exceed
+ * the limit by |c qdd_t| (an exact saturating solve would need an active-set iteration).  For a non-symmetric inertia_mat
+ * the arithmetic above is the definition.
  */
 int drmb200_pd_rollout(const drmb200_topology_t* topo, const float* table,
                        const float* q0, const float* qd0, const float* q_ref, const float* qd_ref, const float* f,
@@ -370,6 +395,13 @@ int drmb200_pd_rollout(const drmb200_topology_t* topo, const float* table,
  * (q_t, qd_t, tau_t) (the implicit-damping adjoint under DRMB200_IMPLICIT_DAMPING), with one element-wise launch per
  * step between them (2 n_steps + 2 launches, no atomics: bitwise reproducible).  `workspace` must hold drmb200_pd_rollout_backward_workspace_bytes(topo, batch) bytes; it does not depend
  * on n_steps.  Outputs must not alias inputs.
+ * DRMB200_IMPLICIT_GAINS: the adjoint of that step, still 2 n_steps + 2 launches without atomics.  Each element-wise
+ * launch recomputes u^_t, sat_t, u_t and c_t bit-exactly from (q_t, qd_t) and the ABA adjoint runs at (q_t, qd_t, u_t)
+ * with the pivot addends c_t, returning their adjoint c-bar and its recomputed qdd_t as well; with mask = !sat,
+ * gu = mask (f-bar + g_tau) and gc = mask (c-bar - qdd_t g_tau), the feedback terms become a_q -= kp gu,
+ * a_qd -= (kd + h kp) gu, kp_grad += gu e + h^2 gc, kd_grad += gu ed + h gc (q_ref_grad = kp gu, qd_ref_grad = kd gu,
+ * f_grad = gu), and g_qdd_t gets -c_t g_tau[t].  The workspace bound covers this case too: it is larger than before the
+ * flag existed, by four [B, n_dofs] fp32 slices.
  */
 int64_t drmb200_pd_rollout_backward_workspace_bytes(const drmb200_topology_t* topo, int64_t batch);
 int drmb200_pd_rollout_backward(const drmb200_topology_t* topo, const float* table,
